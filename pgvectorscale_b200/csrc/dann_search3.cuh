@@ -553,9 +553,13 @@ struct LeanWarp {
 
     /* Hash flavour: a 4-byte entry names its node through its hash slot.  The root the pop leaves behind is the likeliest
      * next visit (about two visits in three), so its node id is fetched right after the pop, asynchronously into shared
-     * memory, and root_after_page finds it there instead of paying a dependent HBM load in front of the neighbour row. */
+     * memory, and root_after_page finds it there instead of paying a dependent HBM load in front of the neighbour row.
+     * The PTX ISA orders two cp.async only through a wait, and the previous visit's copy to the same word may still be
+     * in flight: neither root_after_page (the page minimum became the root) nor push_page_staged (no staged ancestors)
+     * waited for it.  So it is waited for first; it landed a whole visit ago, the wait costs nothing. */
     __device__ __forceinline__ void root_node_async() {
         if (slotpay && heap_len > 0) {
+            dann_cp_async_wait_all();
             if (lane == 0) dann_cp_async(rootnode, hash + T::seq(heap.get_sm(1)));
             dann_cp_async_commit();
         }
@@ -706,6 +710,7 @@ struct LeanWarp {
             scount++;
             if (scount == a.c_target) done = true;
         }
+        if (slotpay) dann_cp_async_wait_all(); /* no copy of this query's root node id outlives it */
         if (a.bitmap_words) { /* leave the bitmap all zero for the slot's next query */
             __syncwarp();
             const uint4 z = make_uint4(0, 0, 0, 0);

@@ -66,6 +66,13 @@ def test_edge_case_fuzz_with_the_lean_kernel_tiny_heaps_and_retries():
     assert passed == 120 + 12     # the seeds + the four reference-KAT cases and the eight medium cases in the same file
 
 
+def test_lean_kernel_instantiations_pass_under_emulation():
+    """tests/test_zz_l_lean_gpu.py: every instantiation of the lean kernel forced through the hooks, and the default plan
+    on both sides of the lean threshold, in shuffled fiber order; the 2^21-node cases need the GPU graph builder."""
+    passed, out = _run(["tests/test_zz_l_lean_gpu.py", "-k", "not gpu_built"], {"SIMT_SCHED": "2"})
+    assert passed == 25 and "skipped" not in out.splitlines()[-1], out[-500:]
+
+
 def test_address_sanitizer_finds_nothing_in_host_code_or_kernels():
     """The emulated ABI built with -fsanitize=address: every "device" buffer is a red-zoned host allocation, so an
     out-of-bounds access by a kernel (or by the host code around it) aborts the run.  Edge-case fuzz with the measured
