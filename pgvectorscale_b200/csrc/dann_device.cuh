@@ -32,6 +32,8 @@
 #define DANN_ST_HEAP 1u
 #define DANN_ST_HASH 2u
 #define DANN_ST_VIS 4u
+// the two-warp kernel's heap warp popped another node than the memory warp predicted (never retried: an internal error)
+#define DANN_ST_INTERNAL 8u
 
 struct IndexView {
     uint32_t n, dim, dim_index, bits, words, cw, R, Rp;

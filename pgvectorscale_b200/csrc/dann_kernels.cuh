@@ -14,6 +14,7 @@
 #include "dann_device.cuh"
 #include "dann_distance.cuh"
 #include "dann_heap.cuh"
+#include "dann_search_common.cuh"
 
 /* f32::NAN (0x7fc00000): the "no distance" value of padded / unrescored rows */
 #define DANN_NAN_F __int_as_float(0x7fc00000)
@@ -426,11 +427,8 @@ __global__ void dann_check_unique_kernel(const uint32_t *nbrs, uint32_t n, uint3
         const uint32_t *r = nbrs + (size_t)row * Rp;
         uint32_t n0 = lane < R ? r[lane] : DANN_INVALID_NODE;
         uint32_t n1 = lane + 32 < R ? r[lane + 32] : DANN_INVALID_NODE;
-        unsigned i0 = __ballot_sync(DANN_FULL, n0 == DANN_INVALID_NODE);
-        unsigned i1 = __ballot_sync(DANN_FULL, n1 == DANN_INVALID_NODE);
-        uint32_t cut0 = i0 ? (uint32_t)(__ffs(i0) - 1) : 32u;
-        uint32_t cut1 = i0 ? 0u : (i1 ? (uint32_t)(__ffs(i1) - 1) : 32u);
-        bool v0 = lane < cut0, v1 = lane < cut1;
+        bool v0, v1;
+        neighbour_cut(n0, n1, (int)lane, v0, v1);
         if (!v0) n0 = DANN_INVALID_NODE;
         if (!v1) n1 = DANN_INVALID_NODE;
         const unsigned mm0 = __match_any_sync(DANN_FULL, n0), mm1 = __match_any_sync(DANN_FULL, n1);

@@ -1,14 +1,19 @@
 // dann_plan.h — host-side planning of the search kernels' per-query workspace and launch shape.
 //
 // Pure host arithmetic (no CUDA calls), shared by the C ABI implementation (diskann_b200.cu) and by the CPU
-// SIMT-emulation harness under tests/simt, so that the emulated kernels run with exactly the shapes the
-// product launches.  Include after dann_search2.cuh (sizeof(PairCtl), DANN_LIST_CAP).
+// SIMT-emulation harness under tests/simt, so that the emulated kernels run with exactly the shapes and arguments the
+// product launches.  It lays out the shared memory of all three search kernels, so it includes their headers
+// (DANN_LIST_CAP and SearchArgs of dann_search_common.cuh, sizeof(PairCtl), DANN_STG_CAP).
 #pragma once
 #include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
 
 #include <algorithm>
+
+#include "dann_search.cuh"
+#include "dann_search2.cuh"
+#include "dann_search3.cuh"
 
 struct SearchPlan {
     uint32_t need, cand_cap, hash_cap, vcap, hs, W, grid, per_warp, esize, bitmap_words, ins_cap;
@@ -184,4 +189,22 @@ static int dann_make_plan(const PlanInputs &in, uint32_t nq, uint32_t L, uint32_
     p->per_warp = (uint32_t)((fixed + (size_t)hs * p->esize + 15) & ~(size_t)15);
     p->grid = std::min<uint32_t>((uint32_t)in.sm_count, (nq + W - 1) / W);
     return DANN_OK;
+}
+
+/* The launch arguments every search kernel takes from the index (its view, code mapping and list check) and from the
+ * plan; the caller adds its request, its buffers and its mode. */
+static SearchArgs search_args_for_plan(const IndexView &v, uint32_t G, uint32_t Gshift, uint32_t lists_unique, const SearchPlan &p) {
+    SearchArgs a;
+    a.ix = v;
+    a.G = G;
+    a.Gshift = Gshift;
+    a.lists_unique = lists_unique;
+    a.hash_cap = p.hash_cap;
+    a.bitmap_words = p.bitmap_words;
+    a.ins_cap = p.ins_cap;
+    a.cand_cap = p.cand_cap;
+    a.hs = p.hs;
+    a.vcap = p.vcap;
+    a.per_warp_smem = p.per_warp;
+    return a;
 }

@@ -35,87 +35,10 @@
 // decreases during pushes) and write those directly; the rest are sifted one at a time, in
 // order, by the warp-cooperative sift-up of dann_heap.cuh (one lane per tree level).
 #pragma once
-#include "dann_device.cuh"
+#include "dann_search_common.cuh"
 #include "dann_distance.cuh"
 #include "dann_heap.cuh"
 
-/* what a suspended scan keeps besides its HBM workspace (heap tail, inserted-set, seq->node table) */
-struct SavedScan {
-    uint32_t valid, heap_len, vis_len, ncand, nins, visits, dq, exhausted;
-};
-
-struct SearchArgs {
-    IndexView ix;
-    const uint64_t *q_codes;    /* [B][cw] */
-    const int16_t *q_labels;    /* CSR values, sorted+dedup per query */
-    const int32_t *q_label_off; /* [B+1]; NULL => no scan key (labels None) */
-    const uint32_t *qlist;      /* optional [nq] query ids (retry pass) */
-    uint32_t nq;
-    uint32_t L, c_target;
-    uint32_t *stream;           /* [B][c_target] node ids in consume order */
-    uint32_t *stream_len;       /* [B] */
-    dann_query_stats *stats;    /* [B] */
-    uint32_t *overflow;         /* OR of status bits over all queries of this launch */
-    uint32_t *counter;          /* work-queue head */
-    uint32_t *hash;             /* [slots][hash_cap] (bitmap_words == 0) */
-    uint32_t hash_cap;          /* power of two */
-    uint32_t *bitmap;           /* [slots][bitmap_words], all zero between queries */
-    uint32_t bitmap_words;      /* 0 => use the hash set */
-    uint32_t *ins_list;         /* [slots][ins_cap] inserted ids (bitmap mode: replayed to clear) */
-    uint32_t ins_cap;
-    uint32_t *cand_node;        /* [slots][cand_cap] */
-    uint32_t cand_cap;
-    void *heap_tail;            /* [slots][cand_cap] entries E (indices >= hs used) */
-    uint32_t hs, vcap;
-    uint32_t G, Gshift;         /* lanes per code row (power of two) */
-    uint32_t lists_unique;      /* no neighbour list repeats an id (checked at index load) */
-    uint32_t per_warp_smem;
-    /* resumable scan (dann_scan_gettuple): single query, single warp; the per-scan workspace is not
-     * shared with other queries, so the state below survives between launches */
-    struct SavedScan *saved; /* NULL = one-shot */
-    void *saved_heap_sm;     /* [hs] copy of the shared-memory part of the heap */
-    uint64_t *saved_vis;     /* [vcap] */
-    /* build mode (dann_build.cuh): the scan stops when visit_closest first returns None and the
-     * visited list (graph/mod.rs:285-327 greedy_search_for_build) is written out instead of a stream */
-    uint32_t build_mode;
-    uint64_t *vis_out;      /* [B][vis_out_cap] (dist << 32) | node, ascending */
-    uint32_t *vis_out_len;  /* [B] */
-    uint32_t vis_out_cap;
-    /* engine switches read from DANN_HV_FLAGS (default: all on).  Bit 2 (DANN_HV_POP): the lean kernel's pop walks
-     * the hole down four heap levels per memory round trip (off: lane 0 walks it level by level).  Kept last: the
-     * offsets of the fields above are unchanged. */
-    uint32_t hv_flags;
-    /* plain storage layout (SearchWarp<.., PLAIN=1> only; storage.rs:144-169, plain/storage.rs:223-299): the beam
-     * search compares the query's index slice with the f32 vector each node stores.  Kept after everything else. */
-    const float *plain_vectors; /* [n][plain_dim] */
-    const float *q_index;       /* [B][plain_dim] prepared (truncated, cosine-normalised) queries */
-    uint32_t plain_dim;         /* num_dimensions_to_index */
-};
-#define DANN_HV_POP 2u
-
-#define DANN_LIST_CAP 64u
-
-/* Heap entry layouts: (distance << SEQ_BITS) | candidate sequence number.  Only the distance takes part in
- * comparisons.  Ent32x21: 11-bit distances (codes of up to 2047 bits, e.g. 768-d x 2 bits = 1536) and up
- * to 2M candidates per query in 4 bytes; Ent32x16: 16-bit distances, up to 65536 candidates; Ent64: anything. */
-struct Ent32x21 {
-    using E = uint32_t;
-    static constexpr int KSHIFT = 21;
-    static __device__ __forceinline__ uint32_t make(uint32_t d, uint32_t seq) { return (d << 21) | seq; }
-    static __device__ __forceinline__ uint32_t seq(uint32_t e) { return e & 0x1FFFFFu; }
-};
-struct Ent32x16 {
-    using E = uint32_t;
-    static constexpr int KSHIFT = 16;
-    static __device__ __forceinline__ uint32_t make(uint32_t d, uint32_t seq) { return (d << 16) | seq; }
-    static __device__ __forceinline__ uint32_t seq(uint32_t e) { return e & 0xFFFFu; }
-};
-struct Ent64 {
-    using E = uint64_t;
-    static constexpr int KSHIFT = 32;
-    static __device__ __forceinline__ uint64_t make(uint32_t d, uint32_t seq) { return ((uint64_t)d << 32) | seq; }
-    static __device__ __forceinline__ uint32_t seq(uint64_t e) { return (uint32_t)e; }
-};
 /* PLAIN = 1: the plain storage layout.  Keys are total_ukey(f32 distance) (Ent64 entries), every comparison is a
  * full-distance comparison (counted as d_full), there is no label filter (plain/storage.rs:260). */
 template <typename T, int NCH, int PLAIN = 0>
@@ -136,34 +59,12 @@ struct SearchWarp {
     float *qrow; /* PLAIN: this query's index slice in shared memory */
     /* query */
     ulonglong2 qc[NCH];
-    const int16_t *ql;
-    uint32_t nql;
-    bool filter;
+    QueryLabels key;
     /* warp-uniform state */
     uint32_t heap_len, vis_head, vis_len, ncand, nins, listn;
     uint32_t visits, dq, status;
 
     __device__ __forceinline__ SearchWarp(const SearchArgs &a_, int lane_) : a(a_), lane(lane_) {}
-
-    /* prepare_insert: HashSet::insert (graph/mod.rs:126-128), hash-set flavour */
-    __device__ __forceinline__ bool hash_insert(uint32_t n) {
-        const uint32_t mask = a.hash_cap - 1;
-        uint32_t h = (n * 2654435761u) >> (32 - __popc(mask));
-        for (uint32_t probe = 0; probe <= mask; probe++) {
-            uint32_t old = atomicCAS(hash + h, DANN_INVALID_NODE, n);
-            if (old == DANN_INVALID_NODE) return true;
-            if (old == n) return false;
-            h = (h + 1) & mask;
-        }
-        return false;
-    }
-
-    __device__ __forceinline__ bool node_passes_filter(uint32_t n) {
-        /* labels.overlaps(node_neighbor.get_labels()), sbq/storage.rs:165-172 */
-        if (!a.ix.has_labels) return false;
-        uint32_t o0 = __ldg(a.ix.label_off + n), o1 = __ldg(a.ix.label_off + n + 1);
-        return labels_overlap(ql, nql, a.ix.labels + o0, o1 - o0);
-    }
 
     /* ---- stage: dedupe + label filter of up to 64 neighbour ids (two per lane: list slots
      * `lane` and `lane+32`), appended to the staging list in list order.
@@ -186,9 +87,9 @@ struct SearchWarp {
             new0 = f0 && !(o0 & b0);
             new1 = f1 && !(o1 & b1);
         } else {
-            if (f0) new0 = hash_insert(n0);
+            if (f0) new0 = hash_insert(hash, a.hash_cap, n0);
             __syncwarp();
-            if (f1) new1 = hash_insert(n1);
+            if (f1) new1 = hash_insert(hash, a.hash_cap, n1);
         }
         const unsigned lt = (1u << lane) - 1u;
         const unsigned nm0 = __ballot_sync(DANN_FULL, new0), nm1 = __ballot_sync(DANN_FULL, new1);
@@ -213,8 +114,8 @@ struct SearchWarp {
         }
         bool p0 = new0, p1 = new1;
         if (apply_filter) {
-            if (new0) p0 = node_passes_filter(n0);
-            if (new1) p1 = node_passes_filter(n1);
+            if (new0) p0 = node_passes_filter(a.ix, key, n0);
+            if (new1) p1 = node_passes_filter(a.ix, key, n1);
         }
         const unsigned pm0 = __ballot_sync(DANN_FULL, p0), pm1 = __ballot_sync(DANN_FULL, p1);
         const uint32_t t0 = __popc(pm0), t1 = __popc(pm1);
@@ -346,27 +247,18 @@ struct SearchWarp {
     /* ---- expand one visited node: sbq/storage.rs:135-190.  n0/n1 = list slots lane, lane+32
      * (already loaded by the caller so that the HBM latency overlaps the heap pop). */
     __device__ __forceinline__ void expand(uint32_t v, uint32_t n0, uint32_t n1) {
-        const uint32_t *row = a.ix.nbrs + (size_t)v * a.ix.Rp;
-        const uint32_t R = a.ix.R;
-        for (uint32_t base = 0; base < R && !status; base += 64) {
-            if (base) {
-                n0 = base + lane < R ? ldg_stream_u32(row + base + lane) : DANN_INVALID_NODE;
-                n1 = base + 32 + lane < R ? ldg_stream_u32(row + base + 32 + lane) : DANN_INVALID_NODE;
-            }
-            /* iter_neighbors stops at the first InvalidBlockNumber slot (sbq/node.rs:261-285) */
-            const unsigned i0 = __ballot_sync(DANN_FULL, n0 == DANN_INVALID_NODE);
-            const unsigned i1 = __ballot_sync(DANN_FULL, n1 == DANN_INVALID_NODE);
-            const uint32_t cut0 = i0 ? (uint32_t)(__ffs(i0) - 1) : 32u;
-            const uint32_t cut1 = i0 ? 0u : (i1 ? (uint32_t)(__ffs(i1) - 1) : 32u);
-            const bool v0 = (uint32_t)lane < cut0, v1 = (uint32_t)lane < cut1;
+        for (uint32_t base = 0; base < a.ix.R && !status; base += 64) {
+            if (base) fetch_neighbours(a.ix, v, base, lane, n0, n1);
+            bool v0, v1;
+            const bool ends = neighbour_cut(n0, n1, lane, v0, v1);
             if (a.lists_unique) {
-                stage(n0, v0, n1, v1, filter);
+                stage(n0, v0, n1, v1, key.filter);
             } else { /* a list may repeat an id: keep strict list order across the two chunks */
-                stage(n0, v0, DANN_INVALID_NODE, false, filter);
-                if (!status) stage(n1, v1, DANN_INVALID_NODE, false, filter);
+                stage(n0, v0, DANN_INVALID_NODE, false, key.filter);
+                if (!status) stage(n1, v1, DANN_INVALID_NODE, false, key.filter);
             }
             flush();
-            if (i0 || i1) break;
+            if (ends) break;
         }
     }
 
@@ -442,42 +334,14 @@ struct SearchWarp {
                 qc[i] = c < nchunks ? qrow[c] : make_ulonglong2(0, 0);
             }
         }
-        /* inserted = HashSet::new() (the bitmap flavour is already all zero) */
-        if (!a.bitmap_words && !resumed) {
-            uint4 ff = make_uint4(DANN_INVALID_NODE, DANN_INVALID_NODE, DANN_INVALID_NODE, DANN_INVALID_NODE);
-            uint4 *h4 = reinterpret_cast<uint4 *>(hash);
-            for (uint32_t i = lane; i < a.hash_cap / 4; i += 32) h4[i] = ff;
-            __threadfence_block();
-            __syncwarp();
-        }
-        ql = nullptr;
-        nql = 0;
-        filter = false;
-        if (a.q_label_off) {
-            int32_t o0 = a.q_label_off[q], o1 = a.q_label_off[q + 1];
-            ql = a.q_labels + o0;
-            nql = (uint32_t)(o1 - o0);
-            filter = nql > 0; /* has_label_filter, scan.rs:189 */
-        }
+        if (!a.bitmap_words && !resumed) hash_set_clear(hash, a.hash_cap, lane);
+        key = query_labels(a, q);
         /* greedy_search_streaming_init + ListSearchResult::new (graph/mod.rs:97-124,331-354) */
         if (ix.start_default != DANN_INVALID_NODE && !resumed) {
-            if (a.q_label_off) { /* StartNodes::get_for_node(Some(labels)), start_nodes.rs:39-48 */
-                for (uint32_t b = 0; b < nql && !status; b += 32) {
-                    uint32_t i = b + lane, n = DANN_INVALID_NODE;
-                    bool valid = false;
-                    if (i < nql) {
-                        int16_t lab = __ldg(ql + i);
-                        uint32_t lo = 0, hi = ix.n_start_labels;
-                        while (lo < hi) {
-                            uint32_t mid = (lo + hi) >> 1;
-                            if (__ldg(ix.start_labels + mid) < lab) lo = mid + 1;
-                            else hi = mid;
-                        }
-                        if (lo < ix.n_start_labels && __ldg(ix.start_labels + lo) == lab) {
-                            n = __ldg(ix.start_label_nodes + lo);
-                            valid = true;
-                        }
-                    }
+            if (a.q_label_off) {
+                for (uint32_t b = 0; b < key.n && !status; b += 32) {
+                    uint32_t n;
+                    const bool valid = label_start_node(ix, key, b + lane, n);
                     /* start nodes are not label-checked (storage.rs:365-391) */
                     stage(n, valid, DANN_INVALID_NODE, false, false);
                     flush();
@@ -509,9 +373,8 @@ struct SearchWarp {
                  * first, then let the sift-down and the visited insert run under that latency */
                 const uint32_t d = H::key(head);
                 const uint32_t node = __ldcg(cnode + T::seq(head));
-                const uint32_t *row = ix.nbrs + (size_t)node * ix.Rp;
-                const uint32_t n0 = (uint32_t)lane < ix.R ? ldg_stream_u32(row + lane) : DANN_INVALID_NODE;
-                const uint32_t n1 = (uint32_t)lane + 32 < ix.R ? ldg_stream_u32(row + 32 + lane) : DANN_INVALID_NODE;
+                uint32_t n0, n1;
+                fetch_neighbours(ix, node, 0, lane, n0, n1);
                 if (heap_len <= heap.hs) {
                     ArrayStore<E> sm{heap.sm};
                     H::pop_warp(sm, heap_len, lane);
@@ -530,9 +393,9 @@ struct SearchWarp {
             __syncwarp();
             vis_head++;
             vis_len--;
-            uint32_t node = (uint32_t)e;
-            uint64_t tid = __ldg(ix.tids + node); /* return_lsn, sbq/storage.rs:404-414 */
-            if ((tid & 0xFFFFull) == 0) continue; /* InvalidOffsetNumber: deleted tuple, scan.rs:231-234 */
+            const uint32_t node = (uint32_t)e;
+            const uint64_t tid = __ldg(ix.tids + node); /* return_lsn, sbq/storage.rs:404-414 */
+            if ((tid & 0xFFFFull) == 0) continue;       /* InvalidOffsetNumber: deleted tuple, scan.rs:231-234 */
             if (lane == 0) a.stream[(size_t)q * a.c_target + scount] = node;
             scount++;
             if (scount == a.c_target) done = true;
@@ -560,19 +423,7 @@ struct SearchWarp {
             for (uint32_t i = lane; i < nins; i += 32) bitmap[ins[i] >> 5] = 0u;
             __threadfence_block();
         }
-        if (lane == 0) {
-            a.stream_len[q] = scount;
-            dann_query_stats st;
-            st.visits = visits;
-            st.d_quantized = PLAIN == 1 ? 0u : dq;
-            st.candidates = dq;
-            st.d_full = PLAIN == 1 ? dq : 0u; /* record_full_distance_comparison, plain/storage.rs:238,288 */
-            st.stream_len = scount;
-            st.status = status;
-            a.stats[q] = st;
-            if (status) atomicOr(a.overflow, status);
-        }
-        __syncwarp();
+        write_query_stats(a, q, lane, scount, visits, dq, PLAIN == 1, status);
     }
 };
 
@@ -596,11 +447,5 @@ __global__ void __launch_bounds__(384, 1) dann_search_kernel(const SearchArgs a)
     w.heap.sm = hsm;
     w.heap.gl = reinterpret_cast<E *>(a.heap_tail) + (size_t)slot * a.cand_cap;
     w.heap.hs = a.hs;
-    for (;;) {
-        uint32_t qi = 0;
-        if (lane == 0) qi = atomicAdd(a.counter, 1u);
-        qi = __shfl_sync(DANN_FULL, qi, 0);
-        if (qi >= a.nq) break;
-        w.run(a.qlist ? a.qlist[qi] : qi);
-    }
+    serve_queries(a, lane, w);
 }

@@ -24,9 +24,8 @@
 // Hand-off: double-buffered (list, dist) pages and control words in shared memory, one named
 // barrier (bar.sync id, 64) per visit.
 #pragma once
-#include "dann_search.cuh"
-
-#define DANN_ST_INTERNAL 8u
+#include "dann_search_common.cuh"
+#include "dann_heap.cuh"
 
 struct PairCtl {
     uint32_t q;             /* query id for this round, 0xFFFFFFFF = no more work */
@@ -84,18 +83,6 @@ struct PairSearch {
     uint32_t vis_head, vis_len; /* the visited list belongs to the controller (memory) warp */
     bool filter;
 
-    __device__ __forceinline__ bool hash_insert(uint32_t n) {
-        const uint32_t mask = a.hash_cap - 1;
-        uint32_t h = (n * 2654435761u) >> (32 - __popc(mask));
-        for (uint32_t probe = 0; probe <= mask; probe++) {
-            uint32_t old = atomicCAS(hash + h, DANN_INVALID_NODE, n);
-            if (old == DANN_INVALID_NODE) return true;
-            if (old == n) return false;
-            h = (h + 1) & mask;
-        }
-        return false;
-    }
-
     __device__ __forceinline__ bool node_passes_filter(uint32_t n) {
         if (!a.ix.has_labels) return false;
         uint32_t o0 = __ldg(a.ix.label_off + n), o1 = __ldg(a.ix.label_off + n + 1);
@@ -142,9 +129,9 @@ struct PairSearch {
             new0 = f0 && !(o0 & b0);
             new1 = f1 && !(o1 & b1);
         } else {
-            if (f0) new0 = hash_insert(n0);
+            if (f0) new0 = hash_insert(hash, a.hash_cap, n0);
             __syncwarp();
-            if (f1) new1 = hash_insert(n1);
+            if (f1) new1 = hash_insert(hash, a.hash_cap, n1);
         }
         const unsigned lt = (1u << lane) - 1u;
         const unsigned nm0 = __ballot_sync(DANN_FULL, new0), nm1 = __ballot_sync(DANN_FULL, new1);
@@ -414,19 +401,7 @@ struct PairSearch {
             for (; i < nins; i += 32) bitmap[ins[i] >> 5] = 0u;
             __threadfence_block();
         }
-        if (lane == 0) {
-            a.stream_len[q] = scount;
-            dann_query_stats st;
-            st.visits = visits;
-            st.d_quantized = ncand; /* every staged candidate was pushed */
-            st.candidates = ncand;
-            st.d_full = 0;
-            st.stream_len = scount;
-            st.status = status;
-            a.stats[q] = st;
-            if (status) atomicOr(a.overflow, status);
-        }
-        __syncwarp();
+        write_query_stats(a, q, lane, scount, visits, ncand, false, status); /* every staged candidate was pushed */
     }
 
     /* ================================= heap warp ======================================= */

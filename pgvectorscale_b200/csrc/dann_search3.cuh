@@ -29,7 +29,8 @@
 // [64] u32, page of entries [64] E, staging area of the pushes [160] E.  HBM per slot: heap tail [cand_cap] E, inserted-set (bitmap n/8 bytes, or
 // hash_cap u32).
 #pragma once
-#include "dann_search.cuh"
+#include "dann_search_common.cuh"
+#include "dann_heap.cuh"
 
 /* staged slots of one page of pushes: tn leaves + (tn/2 + 1) + (tn/4 + 1) + ... <= 2 tn + 32 */
 #define DANN_STG_CAP (2u * DANN_LIST_CAP + 32u)
@@ -53,9 +54,8 @@ struct LeanWarp {
     SplitStore<E> heap; /* 1-based: Rust's data[i] is slot i + 1 */
     ulonglong2 *qcode; /* [NCH * G] 16-byte chunks of the query's SBQ code, zero past the code's end */
     uint32_t *rootnode; /* hash flavour: node id of the heap's root as the last pop left it (filled by cp.async) */
-    const int16_t *ql;
-    uint32_t nql;
-    bool filter, slotpay;
+    QueryLabels key;
+    bool slotpay;
     uint32_t heap_len, vis_head, vis_len, nset, listn, visits, dq, status;
 
     __device__ __forceinline__ LeanWarp(const SearchArgs &a_, int lane_) : a(a_), lane(lane_) {}
@@ -63,13 +63,6 @@ struct LeanWarp {
     __device__ __forceinline__ uint32_t node_of(E e) const {
         const uint32_t p = T::seq(e);
         return slotpay ? __ldcg(hash + p) : p;
-    }
-
-    __device__ __forceinline__ bool node_passes_filter(uint32_t n) {
-        /* labels.overlaps(node_neighbor.get_labels()), sbq/storage.rs:165-172 */
-        if (!a.ix.has_labels) return false;
-        const uint32_t o0 = __ldg(a.ix.label_off + n), o1 = __ldg(a.ix.label_off + n + 1);
-        return labels_overlap(ql, nql, a.ix.labels + o0, o1 - o0);
     }
 
     /* prepare_insert = HashSet::insert (graph/mod.rs:126-128) of up to 64 neighbour ids (list slots `lane` and
@@ -154,8 +147,8 @@ struct LeanWarp {
         }
         bool p0 = new0, p1 = new1;
         if (apply_filter) {
-            if (new0) p0 = node_passes_filter(n0);
-            if (new1) p1 = node_passes_filter(n1);
+            if (new0) p0 = node_passes_filter(a.ix, key, n0);
+            if (new1) p1 = node_passes_filter(a.ix, key, n1);
         }
         const unsigned lt = (1u << lane) - 1u;
         const unsigned pm0 = __ballot_sync(DANN_FULL, p0), pm1 = __ballot_sync(DANN_FULL, p1);
@@ -501,27 +494,23 @@ struct LeanWarp {
      * depend on them - runs under their round trip.  Leaves the page (ids + entries with distances) staged: the
      * caller pushes it.  Returns the page length. */
     __device__ __forceinline__ uint32_t visit(E head, uint32_t n0, uint32_t n1) {
-        /* iter_neighbors stops at the first InvalidBlockNumber slot (sbq/node.rs:261-285) */
-        const unsigned i0 = __ballot_sync(DANN_FULL, n0 == DANN_INVALID_NODE);
-        const unsigned i1 = __ballot_sync(DANN_FULL, n1 == DANN_INVALID_NODE);
-        const uint32_t cut0 = i0 ? (uint32_t)(__ffs(i0) - 1) : 32u;
-        const uint32_t cut1 = i0 ? 0u : (i1 ? (uint32_t)(__ffs(i1) - 1) : 32u);
-        const bool v0 = (uint32_t)lane < cut0, v1 = (uint32_t)lane < cut1;
+        bool v0, v1;
+        neighbour_cut(n0, n1, lane, v0, v1);
         if (a.lists_unique) {
             const Probe pr = stage_probe(n0, v0, n1, v1, true);
             pop();
             root_node_async();
             visited_insert(head);
             if (status) return 0;
-            stage_tail(pr, n0, n1, filter);
+            stage_tail(pr, n0, n1, key.filter);
         } else {
             pop();
             root_node_async();
             visited_insert(head);
             if (status) return 0;
             /* a list may repeat an id: keep strict list order across the two chunks */
-            stage(n0, v0, DANN_INVALID_NODE, false, filter, false);
-            if (!status) stage(n1, v1, DANN_INVALID_NODE, false, filter, false);
+            stage(n0, v0, DANN_INVALID_NODE, false, key.filter, false);
+            if (!status) stage(n1, v1, DANN_INVALID_NODE, false, key.filter, false);
         }
         const uint32_t tn = listn;
         listn = 0;
@@ -622,42 +611,14 @@ struct LeanWarp {
             for (uint32_t c = lane; c < padded; c += 32) qcode[c] = c < nchunks ? qrow[c] : make_ulonglong2(0, 0);
             __syncwarp();
         }
-        if (!a.bitmap_words) { /* inserted = HashSet::new() (the bitmap flavour is left all zero by the previous query) */
-            const uint4 ff = make_uint4(DANN_INVALID_NODE, DANN_INVALID_NODE, DANN_INVALID_NODE, DANN_INVALID_NODE);
-            uint4 *h4 = reinterpret_cast<uint4 *>(hash);
-            for (uint32_t i = lane; i < a.hash_cap / 4; i += 32) h4[i] = ff;
-            __threadfence_block();
-            __syncwarp();
-        }
-        ql = nullptr;
-        nql = 0;
-        filter = false;
-        if (a.q_label_off) {
-            const int32_t o0 = a.q_label_off[q], o1 = a.q_label_off[q + 1];
-            ql = a.q_labels + o0;
-            nql = (uint32_t)(o1 - o0);
-            filter = nql > 0; /* has_label_filter, scan.rs:189 */
-        }
+        if (!a.bitmap_words) hash_set_clear(hash, a.hash_cap, lane);
+        key = query_labels(a, q);
         /* greedy_search_streaming_init + ListSearchResult::new (graph/mod.rs:97-124,331-354) */
         if (ix.start_default != DANN_INVALID_NODE) {
-            if (a.q_label_off) { /* StartNodes::get_for_node(Some(labels)), start_nodes.rs:39-48 */
-                for (uint32_t b = 0; b < nql && !status; b += 32) {
-                    const uint32_t i = b + lane;
-                    uint32_t n = DANN_INVALID_NODE;
-                    bool valid = false;
-                    if (i < nql) {
-                        const int16_t lab = __ldg(ql + i);
-                        uint32_t lo = 0, hi = ix.n_start_labels;
-                        while (lo < hi) {
-                            const uint32_t mid = (lo + hi) >> 1;
-                            if (__ldg(ix.start_labels + mid) < lab) lo = mid + 1;
-                            else hi = mid;
-                        }
-                        if (lo < ix.n_start_labels && __ldg(ix.start_labels + lo) == lab) {
-                            n = __ldg(ix.start_label_nodes + lo);
-                            valid = true;
-                        }
-                    }
+            if (a.q_label_off) {
+                for (uint32_t b = 0; b < key.n && !status; b += 32) {
+                    uint32_t n;
+                    const bool valid = label_start_node(ix, key, b + lane, n);
                     /* start nodes are not label-checked (storage.rs:365-391); two labels may share a start node */
                     stage(n, valid, DANN_INVALID_NODE, false, false, false);
                     flush();
@@ -677,11 +638,7 @@ struct LeanWarp {
             while (heap_len > 0) {
                 if (!pend) head = heap.get_sm(1);
                 if (!may_visit(head)) break; /* a requested row stays valid: nothing touches the heap until the visit */
-                if (!pend) { /* the popped element IS the current root: fetch its neighbour list */
-                    const uint32_t *row = ix.nbrs + (size_t)node_of(head) * ix.Rp;
-                    n0 = (uint32_t)lane < ix.R ? ldg_stream_u32(row + lane) : DANN_INVALID_NODE;
-                    n1 = (uint32_t)lane + 32 < ix.R ? ldg_stream_u32(row + 32 + lane) : DANN_INVALID_NODE;
-                }
+                if (!pend) fetch_neighbours(ix, node_of(head), 0, lane, n0, n1); /* the popped element IS the current root */
                 pend = false;
                 visits++;
                 const uint32_t tn = visit(head, n0, n1);
@@ -690,11 +647,7 @@ struct LeanWarp {
                  * room in the visited list - and its neighbour row is in flight while the pushes run */
                 uint32_t nnode = 0;
                 pend = root_after_page(tn, &head, &nnode);
-                if (pend) {
-                    const uint32_t *row = ix.nbrs + (size_t)nnode * ix.Rp;
-                    n0 = (uint32_t)lane < ix.R ? ldg_stream_u32(row + lane) : DANN_INVALID_NODE;
-                    n1 = (uint32_t)lane + 32 < ix.R ? ldg_stream_u32(row + 32 + lane) : DANN_INVALID_NODE;
-                }
+                if (pend) fetch_neighbours(ix, nnode, 0, lane, n0, n1);
                 if (tn) push_page(tn);
             }
             if (status) break;
@@ -718,19 +671,7 @@ struct LeanWarp {
             for (uint32_t i = lane; i < a.bitmap_words / 4; i += 32) b4[i] = z;
             __threadfence_block();
         }
-        if (lane == 0) {
-            a.stream_len[q] = scount;
-            dann_query_stats st;
-            st.visits = visits;
-            st.d_quantized = dq;
-            st.candidates = dq;
-            st.d_full = 0u;
-            st.stream_len = scount;
-            st.status = status;
-            a.stats[q] = st;
-            if (status) atomicOr(a.overflow, status);
-        }
-        __syncwarp();
+        write_query_stats(a, q, lane, scount, visits, dq, false, status);
     }
 };
 
@@ -754,11 +695,5 @@ __global__ void __launch_bounds__(MAXW * 32, 1) dann_search3_kernel(const Search
     w.bitmap = a.bitmap + (size_t)slot * a.bitmap_words;
     w.heap.gl = reinterpret_cast<E *>(a.heap_tail) + (size_t)slot * a.cand_cap;
     w.heap.hs = a.hs;
-    for (;;) {
-        uint32_t qi = 0;
-        if (lane == 0) qi = atomicAdd(a.counter, 1u);
-        qi = __shfl_sync(DANN_FULL, qi, 0);
-        if (qi >= a.nq) break;
-        w.run(a.qlist ? a.qlist[qi] : qi);
-    }
+    serve_queries(a, lane, w);
 }

@@ -153,7 +153,7 @@ struct dann_scan {
     int nlabels = -1;
     int L = 100, rescore = 50;
     bool active = false;
-    /* suspended search state in HBM (see SavedScan / dann_search.cuh) */
+    /* suspended search state in HBM (see SavedScan / dann_search_common.cuh) */
     DevBuf d_qindex; /* plain layout: the prepared index slice */
     DevBuf d_step;   /* DANN_SCAN_FUSED: one ScanStepOut per amgettuple */
     DevBuf d_query, d_qfull, d_qcodes, d_labels, d_label_off, d_saved, d_heap_sm, d_vis, d_heap_tail, d_cnode, d_set,
@@ -648,8 +648,7 @@ static int run_search(dann_index *ix, const uint64_t *d_q_codes, const int16_t *
             if (!p.lean) CK(ix->ws_ins.reserve(slots * (size_t)p.ins_cap * 4));
         }
         CK(cudaMemsetAsync(d_ctl, 0, 8, st));
-        SearchArgs a;
-        a.ix = v;
+        SearchArgs a = search_args_for_plan(v, ix->G, ix->Gshift, ix->lists_unique, p);
         a.q_codes = d_q_codes;
         a.q_labels = d_labels;
         a.q_label_off = d_label_off;
@@ -663,23 +662,10 @@ static int run_search(dann_index *ix, const uint64_t *d_q_codes, const int16_t *
         a.overflow = d_ctl + 1;
         a.counter = d_ctl;
         a.hash = ix->ws_hash.as<uint32_t>();
-        a.hash_cap = p.hash_cap;
         a.bitmap = ix->ws_bitmap.as<uint32_t>();
-        a.bitmap_words = p.bitmap_words;
         a.ins_list = ix->ws_ins.as<uint32_t>();
-        a.ins_cap = p.ins_cap;
-        a.lists_unique = ix->lists_unique;
         a.cand_node = ix->ws_cand.as<uint32_t>();
-        a.cand_cap = p.cand_cap;
         a.heap_tail = ix->ws_heap.p;
-        a.hs = p.hs;
-        a.vcap = p.vcap;
-        a.G = ix->G;
-        a.Gshift = ix->Gshift;
-        a.per_warp_smem = p.per_warp;
-        a.saved = nullptr;
-        a.saved_heap_sm = nullptr;
-        a.saved_vis = nullptr;
         a.build_mode = vis_out ? 1u : 0u;
         a.vis_out = vis_out;
         a.vis_out_len = vis_out_len;
@@ -1297,12 +1283,10 @@ static int scan_launch_search(dann_scan *sc, uint32_t want) {
         CK(sc->d_stream.reserve((size_t)want * 4));
         uint32_t *d_ctl = sc->d_ctl.as<uint32_t>();
         CK(cudaMemsetAsync(d_ctl, 0, 8, st));
-        SearchArgs a;
-        a.ix = v;
+        SearchArgs a = search_args_for_plan(v, ix->G, ix->Gshift, ix->lists_unique, p);
         a.q_codes = sc->d_qcodes.as<uint64_t>();
         a.q_labels = sc->nlabels >= 0 ? sc->d_labels.as<int16_t>() : nullptr;
         a.q_label_off = sc->nlabels >= 0 ? sc->d_label_off.as<int32_t>() : nullptr;
-        a.qlist = nullptr;
         a.nq = 1;
         a.L = (uint32_t)sc->L;
         a.c_target = want;
@@ -1312,28 +1296,13 @@ static int scan_launch_search(dann_scan *sc, uint32_t want) {
         a.overflow = d_ctl + 1;
         a.counter = d_ctl;
         a.hash = sc->d_set.as<uint32_t>();
-        a.hash_cap = p.hash_cap;
         a.bitmap = sc->d_set.as<uint32_t>();
-        a.bitmap_words = p.bitmap_words;
         a.ins_list = sc->d_ins.as<uint32_t>();
-        a.ins_cap = p.ins_cap;
-        a.lists_unique = ix->lists_unique;
         a.cand_node = sc->d_cnode.as<uint32_t>();
-        a.cand_cap = p.cand_cap;
         a.heap_tail = sc->d_heap_tail.p;
-        a.hs = p.hs;
-        a.vcap = p.vcap;
-        a.G = ix->G;
-        a.Gshift = ix->Gshift;
-        a.per_warp_smem = p.per_warp;
         a.saved = sc->d_saved.as<SavedScan>();
         a.saved_heap_sm = sc->d_heap_sm.p;
         a.saved_vis = sc->d_vis.as<uint64_t>();
-        a.build_mode = 0;
-        a.vis_out = nullptr;
-        a.vis_out_len = nullptr;
-        a.vis_out_cap = 0;
-        a.hv_flags = 0;
         a.plain_vectors = ix->index_vectors;
         a.q_index = sc->d_qindex.as<float>();
         a.plain_dim = ix->plain ? v.dim_index : 0;

@@ -1,4 +1,4 @@
-// emu_search.cpp — runs the beam-search kernel SOURCES (pgvectorscale_b200/csrc/dann_search{,2}.cuh) under the CPU
+// emu_search.cpp — runs the beam-search kernel SOURCES (pgvectorscale_b200/csrc/dann_search{,2,3}.cuh) under the CPU
 // SIMT emulator with the product's own workspace plan (dann_plan.h), mirroring run_search() in diskann_b200.cu:
 // same launch shape, same overflow/retry loop.  TEST INFRASTRUCTURE ONLY (see simt_emu.h); built by
 // tests/simt/build_emu.py with g++, never by build.py, never loaded by the package.
@@ -185,8 +185,7 @@ extern "C" int emu_search(const dann_snapshot_desc *s, const uint64_t *q_codes, 
         g_ins.init(p.bitmap_words && !p.lean ? slots * (size_t)p.ins_cap * 4 : 16, 0);
         g_heap.init(slots * (size_t)p.cand_cap * p.esize, 0);
         ctl[0] = ctl[1] = 0;
-        SearchArgs a{};
-        a.ix = v;
+        SearchArgs a = search_args_for_plan(v, G, Gshift, lists_unique, p);
         a.q_codes = qc;
         a.q_labels = qlab;
         a.q_label_off = qoff;
@@ -200,20 +199,10 @@ extern "C" int emu_search(const dann_snapshot_desc *s, const uint64_t *q_codes, 
         a.overflow = ctl + 1;
         a.counter = ctl;
         a.hash = reinterpret_cast<uint32_t *>(g_hash.p());
-        a.hash_cap = p.hash_cap;
         a.bitmap = reinterpret_cast<uint32_t *>(g_bitmap.p());
-        a.bitmap_words = p.bitmap_words;
         a.ins_list = reinterpret_cast<uint32_t *>(g_ins.p());
-        a.ins_cap = p.ins_cap;
-        a.lists_unique = lists_unique;
         a.cand_node = reinterpret_cast<uint32_t *>(g_cand.p());
-        a.cand_cap = p.cand_cap;
         a.heap_tail = g_heap.p();
-        a.hs = p.hs;
-        a.vcap = p.vcap;
-        a.G = G;
-        a.Gshift = Gshift;
-        a.per_warp_smem = p.per_warp;
         a.hv_flags = env_u32("DANN_HV_FLAGS", 4095);
         a.plain_vectors = ivp;
         a.q_index = qip;
