@@ -125,6 +125,12 @@ __device__ __forceinline__ int32_t total_key(float f) {
 }
 // same, biased so that unsigned compare gives the total order
 __device__ __forceinline__ uint32_t total_ukey(float f) { return (uint32_t)total_key(f) ^ 0x80000000u; }
+// the float whose total_ukey is k (the sign-dependent xor of total_key is its own inverse)
+__device__ __forceinline__ float total_ukey_inverse(uint32_t k) {
+    int32_t b = (int32_t)(k ^ 0x80000000u);
+    b ^= (int32_t)(((uint32_t)(b >> 31)) >> 1);
+    return __int_as_float(b);
+}
 
 // labels/mod.rs:124-142 LabelSetView::overlaps (two-pointer over two ascending i16 arrays)
 __device__ __forceinline__ bool labels_overlap(const int16_t *a, uint32_t na, const int16_t *b,

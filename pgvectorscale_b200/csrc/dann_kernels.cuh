@@ -1,9 +1,10 @@
 // dann_kernels.cuh — the non-graph kernels of the scan path (sm_90a):
-//   prepare_queries  : amrescan's vector preparation (cosine normalise + SBQ quantize)
+//   prepare / prepare_plain : amrescan's vector preparation (cosine normalise + SBQ quantize)
 //   sbq_distance     : stand-alone batched SBQ XOR+popcount gather (the roofline kernel)
 //   full_distance    : exact f32 L2 / cosine / inner product, AVX2 summation order
-//   rerank_resort    : get_full_distance_for_resort + the sliding rerank window
-//   normalize_rows / pad_rows : index load helpers
+//   rerank           : get_full_distance_for_resort + the sliding rerank window, a batch at a time
+//   scan_distance / scan_finish : the same for the streaming scan, one amgettuple at a time
+//   normalize_rows / pad_rows / check_unique : index load helpers
 // Reference paths are relative to pgvectorscale/src/access_method/.
 // Every f32 operation that decides a result is spelled with an explicit-rounding
 // intrinsic (__fadd_rn, __fmul_rn, __fmaf_rn, __fdiv_rn, __fsqrt_rn): nvcc never
@@ -28,6 +29,32 @@ __device__ __forceinline__ float cosine_divisor_from_norm(float norm, uint32_t l
     if (norm < eps) return 0.0f;
     if (norm >= __fsub_rn(1.0f, adj) && norm <= __fadd_rn(1.0f, adj)) return 0.0f;
     return __fsqrt_rn(norm);
+}
+
+/* amrescan's two cosine divisors of query row `src` (pg_vector.rs:125-157): `dfull` for the full copy of `dim` values,
+ * `dindex` for the copy truncated to `dim_index`; 0 leaves a copy untouched, and always does when !cosine.  Block-wide. */
+__device__ __forceinline__ void query_cosine_divisors(const float *src, uint32_t dim, uint32_t dim_index, bool cosine,
+                                                      float &dfull, float &dindex) {
+    DANN_STATIC_SMEM float s_div[2];
+    if (cosine) {
+        /* Iterator::sum over v*v in index order: a sequential dependent chain; two warps
+         * run the two chains (full copy / truncated copy) side by side. */
+        if (threadIdx.x == 0 || threadIdx.x == 32) {
+            const uint32_t len = threadIdx.x == 0 ? dim : dim_index;
+            float norm = 0.0f;
+            for (uint32_t i = 0; i < len; i++) {
+                float v = src[i];
+                norm = __fadd_rn(norm, __fmul_rn(v, v));
+            }
+            s_div[threadIdx.x >> 5] = cosine_divisor_from_norm(norm, len);
+        }
+    } else if (threadIdx.x == 0) {
+        s_div[0] = 0.0f;
+        s_div[1] = 0.0f;
+    }
+    __syncthreads();
+    dfull = s_div[0];
+    dindex = s_div[1];
 }
 
 /* SbqQuantizer::quantize, one dimension (sbq/quantize.rs:52-102): number of leading ones */
@@ -57,28 +84,10 @@ __global__ void __launch_bounds__(128) dann_prepare_kernel(IndexView ix, const f
                                                            float *q_full_out, uint64_t *q_codes_out) {
     DANN_DYN_SMEM(dann_smem);
     float *qi = reinterpret_cast<float *>(dann_smem); /* [dim_index] normalised index copy */
-    DANN_STATIC_SMEM float s_div[2];
     const int q = blockIdx.x;
     const float *src = queries + (size_t)q * ix.dim;
-    const bool cosine = ix.distance_type == DANN_COSINE;
-    if (cosine) {
-        /* Iterator::sum over v*v in index order: a sequential dependent chain; two warps
-         * run the two chains (full copy / truncated copy) side by side. */
-        if (threadIdx.x == 0 || threadIdx.x == 32) {
-            const uint32_t len = threadIdx.x == 0 ? ix.dim : ix.dim_index;
-            float norm = 0.0f;
-            for (uint32_t i = 0; i < len; i++) {
-                float v = src[i];
-                norm = __fadd_rn(norm, __fmul_rn(v, v));
-            }
-            s_div[threadIdx.x >> 5] = cosine_divisor_from_norm(norm, len);
-        }
-    } else if (threadIdx.x == 0) {
-        s_div[0] = 0.0f;
-        s_div[1] = 0.0f;
-    }
-    __syncthreads();
-    const float dfull = s_div[0], dindex = s_div[1];
+    float dfull, dindex;
+    query_cosine_divisors(src, ix.dim, ix.dim_index, ix.distance_type == DANN_COSINE, dfull, dindex);
     for (uint32_t i = threadIdx.x; i < ix.dim; i += blockDim.x) {
         float v = src[i];
         if (q_full_out) q_full_out[(size_t)q * ix.dim + i] = dfull != 0.0f ? __fdiv_rn(v, dfull) : v;
@@ -107,25 +116,10 @@ __global__ void __launch_bounds__(128) dann_prepare_kernel(IndexView ix, const f
 __global__ void __launch_bounds__(128) dann_prepare_plain_kernel(uint32_t dim, uint32_t dim_index, int cosine,
                                                                  const float *queries, float *q_full_out,
                                                                  float *q_index_out) {
-    DANN_STATIC_SMEM float s_div[2];
     const int q = blockIdx.x;
     const float *src = queries + (size_t)q * dim;
-    if (cosine) {
-        if (threadIdx.x == 0 || threadIdx.x == 32) {
-            const uint32_t len = threadIdx.x == 0 ? dim : dim_index;
-            float norm = 0.0f;
-            for (uint32_t i = 0; i < len; i++) {
-                float v = src[i];
-                norm = __fadd_rn(norm, __fmul_rn(v, v));
-            }
-            s_div[threadIdx.x >> 5] = cosine_divisor_from_norm(norm, len);
-        }
-    } else if (threadIdx.x == 0) {
-        s_div[0] = 0.0f;
-        s_div[1] = 0.0f;
-    }
-    __syncthreads();
-    const float dfull = s_div[0], dindex = s_div[1];
+    float dfull, dindex;
+    query_cosine_divisors(src, dim, dim_index, cosine != 0, dfull, dindex);
     for (uint32_t i = threadIdx.x; i < dim; i += blockDim.x) {
         float v = src[i];
         q_full_out[(size_t)q * dim + i] = dfull != 0.0f ? __fdiv_rn(v, dfull) : v;
@@ -253,6 +247,25 @@ __device__ __forceinline__ void stage_query_row(float *dst, const float *src, ui
     }
 }
 
+/* out[i] = distance_fn(vectors[nodes[i]], qs) for i in [begin, end), begin <= end, with the query row `qs` already
+ * staged in shared memory: 8 lanes per row, 128-bit loads when dim is a multiple of 4.  DANN_INVALID_NODE reads row 0
+ * and gives DANN_NAN_F.  Block-wide. */
+__device__ __forceinline__ void full_distances(const IndexView &ix, const float *qs, const uint32_t *nodes,
+                                               uint32_t begin, uint32_t end, float *out) {
+    const uint32_t lane = threadIdx.x & 31, mm = lane & 7, gbase = lane & 24;
+    const uint32_t group = threadIdx.x >> 3, ngroups = blockDim.x >> 3;
+    const bool vec4 = (ix.dim & 3u) == 0;
+    const uint32_t rounds = (end - begin + ngroups - 1) / ngroups;
+    for (uint32_t r = 0; r < rounds; r++) {
+        const uint32_t it = begin + r * ngroups + group;
+        const uint32_t node = it < end ? nodes[it] : DANN_INVALID_NODE;
+        const float *x = ix.vectors + (size_t)(node == DANN_INVALID_NODE ? 0 : node) * ix.dim;
+        const float d = vec4 ? full_distance_group8<true>(ix.distance_type, x, qs, ix.dim, mm, gbase)
+                             : full_distance_group8<false>(ix.distance_type, x, qs, ix.dim, mm, gbase);
+        if (mm == 0 && it < end) out[it] = node == DANN_INVALID_NODE ? DANN_NAN_F : d;
+    }
+}
+
 /* out[b*m+i] = distance_fn(vectors[nodes[b*m+i]], q_full[b]) ; one CTA per query */
 __global__ void __launch_bounds__(128) dann_full_distance_kernel(IndexView ix, const float *q_full,
                                                                  const uint32_t *nodes, int m, float *out) {
@@ -261,18 +274,7 @@ __global__ void __launch_bounds__(128) dann_full_distance_kernel(IndexView ix, c
     DANN_STATIC_SMEM uint64_t bar;
     const int q = blockIdx.x;
     stage_query_row(qs, q_full + (size_t)q * ix.dim, ix.dim, &bar);
-    const uint32_t lane = threadIdx.x & 31, mm = lane & 7, gbase = lane & 24;
-    const uint32_t group = threadIdx.x >> 3, ngroups = blockDim.x >> 3;
-    const bool vec4 = (ix.dim & 3u) == 0;
-    const uint32_t rounds = ((uint32_t)m + ngroups - 1) / ngroups;
-    for (uint32_t r = 0; r < rounds; r++) {
-        uint32_t it = r * ngroups + group;
-        uint32_t node = it < (uint32_t)m ? nodes[(size_t)q * m + it] : DANN_INVALID_NODE;
-        const float *x = ix.vectors + (size_t)(node == DANN_INVALID_NODE ? 0 : node) * ix.dim;
-        float d = vec4 ? full_distance_group8<true>(ix.distance_type, x, qs, ix.dim, mm, gbase)
-                       : full_distance_group8<false>(ix.distance_type, x, qs, ix.dim, mm, gbase);
-        if (mm == 0 && it < (uint32_t)m) out[(size_t)q * m + it] = node == DANN_INVALID_NODE ? DANN_NAN_F : d;
-    }
+    full_distances(ix, qs, nodes + (size_t)q * m, 0, (uint32_t)m, out + (size_t)q * m);
 }
 
 /* ------------------------------------------------------------------------------------ */
@@ -321,20 +323,7 @@ __global__ void __launch_bounds__(128) dann_rerank_kernel(const RerankArgs a) {
     }
 
     stage_query_row(qs, a.q_full + (size_t)q * ix.dim, ix.dim, &bar);
-    {
-        const uint32_t lane = threadIdx.x & 31, mm = lane & 7, gbase = lane & 24;
-        const uint32_t group = threadIdx.x >> 3, ngroups = blockDim.x >> 3;
-        const bool vec4 = (ix.dim & 3u) == 0;
-        const uint32_t rounds = (sl + ngroups - 1) / ngroups;
-        for (uint32_t r = 0; r < rounds; r++) {
-            uint32_t it = r * ngroups + group;
-            uint32_t node = it < sl ? st[it] : 0u;
-            const float *x = ix.vectors + (size_t)node * ix.dim;
-            float d = vec4 ? full_distance_group8<true>(ix.distance_type, x, qs, ix.dim, mm, gbase)
-                           : full_distance_group8<false>(ix.distance_type, x, qs, ix.dim, mm, gbase);
-            if (mm == 0 && it < sl) ds[it] = d;
-        }
-    }
+    full_distances(ix, qs, st, 0, sl, ds);
     __syncthreads();
     if (threadIdx.x == 0) {
         using H = RustHeap<uint64_t, 32>;
@@ -442,10 +431,12 @@ __global__ void dann_check_unique_kernel(const uint32_t *nbrs, uint32_t n, uint3
 }
 
 /* ------------------------------------------------------------------------------------ */
-/* Streaming scan (dann_scan_gettuple): one step of next_with_resort (scan.rs:244-305).       */
-/* The rerank window lives in HBM between calls: win[] is the BinaryHeap<ResortData> array,   */
-/* entries (total_cmp key of the exact distance << 32) | node.  One thread: push the rows that */
-/* just came off the approximate stream, then pop one row for the executor.                  */
+/* Streaming scan (dann_scan_gettuple): one step of next_with_resort (scan.rs:244-305) per amgettuple, with one host
+ * synchronisation.  The search launch, dann_scan_distance_kernel (exact distances of the rows the search appended) and
+ * dann_scan_finish_kernel (the window step) are enqueued back to back; the two kernels read the search's outcome (rows
+ * produced, overflow bits) from device memory, and the last one gathers everything the host needs into one ScanStepOut.
+ * A search that overflowed its workspace leaves the window alone.  The rerank window lives in HBM between calls: win[]
+ * is the BinaryHeap<ResortData> array, entries (total_cmp key of the exact distance << 32) | node. */
 struct ScanWindow {
     uint32_t len, d_full;
 };
@@ -455,50 +446,6 @@ struct ScanRow {
     float dist;
     uint32_t pad;
 };
-__global__ void dann_scan_resort_kernel(IndexView ix, ScanWindow *w, uint64_t *win, uint32_t rescore,
-                                        const uint32_t *new_nodes, const float *new_dist, uint32_t skip,
-                                        uint32_t nnew, ScanRow *out) {
-    if (threadIdx.x != 0 || blockIdx.x != 0) return;
-    ScanRow r;
-    r.tid = DANN_INVALID_TID;
-    r.node = DANN_INVALID_NODE;
-    r.have = 0;
-    r.dist = DANN_NAN_F;
-    r.pad = 0;
-    if (rescore == 0) { /* resort_buffer.capacity() == 0: the stream order is the result (scan.rs:251-253) */
-        if (nnew > skip) {
-            r.node = new_nodes[skip];
-            r.tid = ix.tids[r.node];
-            r.have = 1;
-        }
-        *out = r;
-        return;
-    }
-    using H = RustHeap<uint64_t, 32>;
-    ArrayStore<uint64_t> store{win};
-    uint32_t len = w->len;
-    for (uint32_t i = skip; i < nnew; i++) { /* full_distance_comparisons += 1; resort_buffer.push(..) */
-        H::push(store, len, ((uint64_t)total_ukey(new_dist[i]) << 32) | new_nodes[i]);
-        w->d_full++;
-    }
-    if (len > 0) {
-        uint64_t e = H::pop(store, len);
-        uint32_t uk = (uint32_t)(e >> 32) ^ 0x80000000u; /* undo total_ukey: the transform is an involution */
-        int32_t b = (int32_t)uk;
-        b ^= (int32_t)(((uint32_t)(b >> 31)) >> 1);
-        r.node = (uint32_t)e;
-        r.dist = __int_as_float(b);
-        r.tid = ix.tids[r.node];
-        r.have = 1;
-    }
-    w->len = len;
-    *out = r;
-}
-
-/* ---- one-synchronisation amgettuple (DANN_SCAN_FUSED=1): the search launch, the exact distances of the rows it
- * appended and the window step are enqueued back to back; the two kernels below read the search's outcome (rows
- * produced, overflow bits) from device memory instead of the host doing so in between, and the last one gathers
- * everything the host needs into one ScanStepOut.  A search that overflowed its workspace leaves the window alone. */
 struct ScanStepOut {
     uint32_t overflow, slen;
     dann_query_stats stats;
@@ -516,18 +463,7 @@ __global__ void __launch_bounds__(128) dann_scan_distance_kernel(IndexView ix, c
     const uint32_t slen = *slen_p;
     if (slen <= skip) return;
     stage_query_row(qs, q_full, ix.dim, &bar);
-    const uint32_t lane = threadIdx.x & 31, mm = lane & 7, gbase = lane & 24;
-    const uint32_t group = threadIdx.x >> 3, ngroups = blockDim.x >> 3;
-    const bool vec4 = (ix.dim & 3u) == 0;
-    const uint32_t m = slen - skip, rounds = (m + ngroups - 1) / ngroups;
-    for (uint32_t r = 0; r < rounds; r++) {
-        const uint32_t it = skip + r * ngroups + group;
-        const uint32_t node = it < slen ? stream[it] : 0u;
-        const float *x = ix.vectors + (size_t)node * ix.dim;
-        const float d = vec4 ? full_distance_group8<true>(ix.distance_type, x, qs, ix.dim, mm, gbase)
-                             : full_distance_group8<false>(ix.distance_type, x, qs, ix.dim, mm, gbase);
-        if (mm == 0 && it < slen) out[it] = d;
-    }
+    full_distances(ix, qs, stream, skip, slen, out);
 }
 
 __global__ void dann_scan_finish_kernel(IndexView ix, ScanWindow *w, uint64_t *win, uint32_t rescore, const uint32_t *stream,
@@ -549,7 +485,7 @@ __global__ void dann_scan_finish_kernel(IndexView ix, ScanWindow *w, uint64_t *w
         return;
     }
     const uint32_t nnew = o.slen;
-    if (rescore == 0) {
+    if (rescore == 0) { /* resort_buffer.capacity() == 0: the stream order is the result (scan.rs:251-253) */
         if (nnew > skip) {
             o.row.node = stream[skip];
             o.row.tid = ix.tids[o.row.node];
@@ -562,17 +498,14 @@ __global__ void dann_scan_finish_kernel(IndexView ix, ScanWindow *w, uint64_t *w
     using H = RustHeap<uint64_t, 32>;
     ArrayStore<uint64_t> store{win};
     uint32_t len = w->len, dfull = w->d_full;
-    for (uint32_t i = skip; i < nnew; i++) {
+    for (uint32_t i = skip; i < nnew; i++) { /* full_distance_comparisons += 1; resort_buffer.push(..) */
         H::push(store, len, ((uint64_t)total_ukey(dist[i]) << 32) | stream[i]);
         dfull++;
     }
     if (len > 0) {
         uint64_t e = H::pop(store, len);
-        uint32_t uk = (uint32_t)(e >> 32) ^ 0x80000000u;
-        int32_t b = (int32_t)uk;
-        b ^= (int32_t)(((uint32_t)(b >> 31)) >> 1);
         o.row.node = (uint32_t)e;
-        o.row.dist = __int_as_float(b);
+        o.row.dist = total_ukey_inverse((uint32_t)(e >> 32));
         o.row.tid = ix.tids[o.row.node];
         o.row.have = 1;
     }

@@ -30,6 +30,21 @@
 /* ------------------------------------------------------------------------------------ */
 #define DANN_SMEM_SLACK 128u /* bytes behind every dynamic shared-memory window (see launch_prepare) */
 
+/* A launch gets at most 48 KB of dynamic shared memory unless its kernel has opted in to more. */
+template <typename K>
+static cudaError_t allow_dynamic_smem(K kernel, size_t bytes) {
+    if (bytes <= 48 * 1024) return cudaSuccess;
+    return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+}
+
+/* LabelSet::from(Vec): sort_unstable + dedup (labels/mod.rs:30-37) of [first, last), appended to `out` */
+static void append_label_set(std::vector<int16_t> &out, const int16_t *first, const int16_t *last) {
+    const size_t s0 = out.size();
+    out.insert(out.end(), first, last);
+    std::sort(out.begin() + s0, out.end());
+    out.erase(std::unique(out.begin() + s0, out.end()), out.end());
+}
+
 static thread_local std::string g_err;
 
 static int fail(int code, const char *fmt, ...) {
@@ -155,9 +170,9 @@ struct dann_scan {
     bool active = false;
     /* suspended search state in HBM (see SavedScan / dann_search_common.cuh) */
     DevBuf d_qindex; /* plain layout: the prepared index slice */
-    DevBuf d_step;   /* DANN_SCAN_FUSED: one ScanStepOut per amgettuple */
+    DevBuf d_step;   /* one ScanStepOut per amgettuple */
     DevBuf d_query, d_qfull, d_qcodes, d_labels, d_label_off, d_saved, d_heap_sm, d_vis, d_heap_tail, d_cnode, d_set,
-        d_ins, d_stream, d_slen, d_stats, d_dist, d_win, d_winst, d_row, d_ctl;
+        d_ins, d_stream, d_slen, d_stats, d_dist, d_win, d_winst, d_ctl;
     SearchPlan plan{};
     uint32_t grow = 1;
     uint32_t streamed = 0;  /* rows taken off the approximate stream so far */
@@ -288,6 +303,20 @@ static int validate_snapshot(const dann_snapshot_desc *s, uint32_t *words_out, b
     return DANN_OK;
 }
 
+/* Cosine heap rows are normalised once, where they arrive: the rerank reads the heap vector through
+ * PgVector::from_datum -> preprocess_cosine (sbq/storage.rs:304-328, pg_vector.rs:153-155), whose result only depends on
+ * the row.  d holds the index's n rows of dim values. */
+static int normalize_rows(dann_index *ix, float *d) {
+    const IndexView &v = ix->v;
+    if (v.distance_type != DANN_COSINE) return DANN_OK;
+    int blocks = std::min<long long>((v.n + 255) / 256, (long long)ix->sm_count * 8);
+    dann_normalize_rows_kernel<<<std::max(blocks, 1), 256, 0, ix->stream>>>(d, v.n, v.dim);
+    ix->launches++;
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(ix->stream));
+    return DANN_OK;
+}
+
 static int index_load_impl(const dann_snapshot_desc *s, const float *index_vectors, int device, dann_index **out) {
     dann_index *ix = nullptr;
     if (!s || !out) return fail(DANN_ERR_INVALID_ARG, "dann_index_load: NULL argument");
@@ -387,15 +416,9 @@ static int index_load_impl(const dann_snapshot_desc *s, const float *index_vecto
         CK(cudaStreamSynchronize(ix->stream));
         ix->lists_unique = h == 0;
     }
-    if (s->distance_type == DANN_COSINE && s->n && vectors) {
-        /* rerank reads the heap vector through PgVector::from_datum -> preprocess_cosine
-         * (sbq/storage.rs:304-328, pg_vector.rs:153-155); the result only depends on the row,
-         * so it is computed once here with the same arithmetic. */
-        int blocks = std::min<long long>((s->n + 255) / 256, (long long)ix->sm_count * 8);
-        dann_normalize_rows_kernel<<<std::max(blocks, 1), 256, 0, ix->stream>>>(vectors, s->n, s->dim);
-        ix->launches++;
-        CK(cudaGetLastError());
-        CK(cudaStreamSynchronize(ix->stream));
+    if (s->n && vectors) {
+        int rc = normalize_rows(ix, vectors);
+        if (rc) return rc;
     }
     guard.keep = true;
     *out = ix;
@@ -442,15 +465,22 @@ static int check_live(dann_index *ix) {
     return DANN_OK;
 }
 
+/* amrescan's vector preparation of B queries: q_full [B][dim], plus the SBQ codes q_codes [B][cw], or for a plain index
+ * the normalised index copy q_index [B][dim_index] */
 static int launch_prepare(dann_index *ix, const float *d_queries, int B, float *d_q_full, uint64_t *d_q_codes,
-                          cudaStream_t st) {
-    /* DANN_SMEM_SLACK: ptxas may turn neighbouring shared-memory loads of a loop into one 16-byte load issued BEFORE the
-     * loop's bounds test (compute-sanitizer caught dann_prepare_kernel reading 16 bytes past a 28-byte window; on
-     * hardware that is a fault whenever it crosses the CTA's allocation), so no dynamic window ends where its data ends */
-    size_t smem = (size_t)((ix->v.dim_index + 3u) & ~3u) * sizeof(float) + DANN_SMEM_SLACK;
-    if (smem > 48 * 1024)
-        CK(cudaFuncSetAttribute(dann_prepare_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    dann_prepare_kernel<<<B, 128, smem, st>>>(ix->v, d_queries, B, d_q_full, d_q_codes);
+                          float *d_q_index, cudaStream_t st) {
+    const IndexView &v = ix->v;
+    if (ix->plain) {
+        dann_prepare_plain_kernel<<<B, 128, 0, st>>>(v.dim, v.dim_index, v.distance_type == DANN_COSINE, d_queries,
+                                                    d_q_full, d_q_index);
+    } else {
+        /* DANN_SMEM_SLACK: ptxas may turn neighbouring shared-memory loads of a loop into one 16-byte load issued BEFORE
+         * the loop's bounds test (compute-sanitizer caught dann_prepare_kernel reading 16 bytes past a 28-byte window; on
+         * hardware that is a fault whenever it crosses the CTA's allocation), so no dynamic window ends where its data ends */
+        size_t smem = (size_t)((v.dim_index + 3u) & ~3u) * sizeof(float) + DANN_SMEM_SLACK;
+        CK(allow_dynamic_smem(dann_prepare_kernel, smem));
+        dann_prepare_kernel<<<B, 128, smem, st>>>(v, d_queries, B, d_q_full, d_q_codes);
+    }
     ix->launches++;
     CK(cudaGetLastError());
     return DANN_OK;
@@ -464,7 +494,7 @@ extern "C" int dann_prepare_queries(dann_index *ix, const float *d_queries, int 
     if (ix->plain) return fail(DANN_ERR_STATE, "dann_prepare_queries: a plain-storage index has no quantizer");
     std::lock_guard<std::mutex> lk(ix->mu);
     DANN_DEVICE_INPUT_STREAM(st, stream);
-    rc = launch_prepare(ix, d_queries, B, d_q_full, d_q_codes, st);
+    rc = launch_prepare(ix, d_queries, B, d_q_full, d_q_codes, nullptr, st);
     if (rc) return rc;
     CK(cudaStreamSynchronize(st));
     return DANN_OK;
@@ -530,8 +560,7 @@ extern "C" int dann_full_distance(dann_index *ix, const float *d_q_full, const u
     if (!d_q_full || !d_nodes || !d_out || B <= 0 || m <= 0) return fail(DANN_ERR_INVALID_ARG, "dann_full_distance: bad argument");
     DANN_DEVICE_INPUT_STREAM(st, stream);
     size_t smem = (size_t)((ix->v.dim + 3u) & ~3u) * sizeof(float) + DANN_SMEM_SLACK;
-    if (smem > 48 * 1024)
-        CK(cudaFuncSetAttribute(dann_full_distance_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CK(allow_dynamic_smem(dann_full_distance_kernel, smem));
     dann_full_distance_kernel<<<B, 128, smem, st>>>(ix->v, d_q_full, d_nodes, m, d_out);
     ix->launches++;
     CK(cudaGetLastError());
@@ -765,17 +794,10 @@ static int search_batch_device_locked(dann_index *ix, const float *d_queries, co
 
     ix->timing = dann_batch_timing{};
     CK(cudaEventRecord(ix->ev[0], st));
-    int rc;
-    if (ix->plain) {
-        CK(ix->sc_qindex.reserve((size_t)B * v.dim_index * sizeof(float)));
-        dann_prepare_plain_kernel<<<B, 128, 0, st>>>(v.dim, v.dim_index, v.distance_type == DANN_COSINE, d_queries,
-                                                    ix->sc_qfull.as<float>(), ix->sc_qindex.as<float>());
-        ix->launches++;
-        CK(cudaGetLastError());
-    } else {
-        rc = launch_prepare(ix, d_queries, B, ix->sc_qfull.as<float>(), ix->sc_qcodes.as<uint64_t>(), st);
-        if (rc) return rc;
-    }
+    if (ix->plain) CK(ix->sc_qindex.reserve((size_t)B * v.dim_index * sizeof(float)));
+    int rc = launch_prepare(ix, d_queries, B, ix->sc_qfull.as<float>(), ix->sc_qcodes.as<uint64_t>(),
+                            ix->sc_qindex.as<float>(), st);
+    if (rc) return rc;
     CK(cudaEventRecord(ix->ev[1], st));
 
     rc = run_search(ix, ix->sc_qcodes.as<uint64_t>(), d_labels, d_label_off, B, (uint32_t)L, c_target, d_stats, nullptr,
@@ -797,8 +819,7 @@ static int search_batch_device_locked(dann_index *ix, const float *d_queries, co
     r.out_count = d_out_count;
     r.stats = d_stats;
     size_t smem = (size_t)((v.dim + 3u) & ~3u) * 4 + (size_t)((c_target + 1u) & ~1u) * 4 + (size_t)rescore * 8 + 16 + DANN_SMEM_SLACK;
-    if (smem > 48 * 1024)
-        CK(cudaFuncSetAttribute(dann_rerank_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    CK(allow_dynamic_smem(dann_rerank_kernel, smem));
     dann_rerank_kernel<<<B, 128, smem, st>>>(r);
     ix->launches++;
     CK(cudaGetLastError());
@@ -858,7 +879,6 @@ static int search_batch_host(dann_index *ix, const float *queries, const int16_t
     std::vector<int16_t> nl;
     std::vector<int32_t> no;
     if (label_off) {
-        /* LabelSet::from(Vec): sort_unstable + dedup per query (labels/mod.rs:30-37) */
         no.resize((size_t)B + 1);
         no[0] = 0;
         if (label_off[0] < 0) return fail(DANN_ERR_INVALID_ARG, "label_off[0] is negative");
@@ -866,10 +886,7 @@ static int search_batch_host(dann_index *ix, const float *queries, const int16_t
         for (int b = 0; b < B; b++) {
             int32_t o0 = label_off[b], o1 = label_off[b + 1];
             if (o1 < o0) return fail(DANN_ERR_INVALID_ARG, "label_off is not monotone");
-            size_t s0 = nl.size();
-            if (o1 > o0) nl.insert(nl.end(), labels + o0, labels + o1);
-            std::sort(nl.begin() + s0, nl.end());
-            nl.erase(std::unique(nl.begin() + s0, nl.end()), nl.end());
+            if (o1 > o0) append_label_set(nl, labels + o0, labels + o1);
             no[b + 1] = (int32_t)nl.size();
         }
         CK(ix->st_labels.reserve(std::max<size_t>(nl.size(), 1) * sizeof(int16_t)));
@@ -922,14 +939,7 @@ extern "C" int dann_index_set_vectors(dann_index *ix, const float *vectors) try 
     }
     CK(cudaMemcpyAsync(d, vectors, (size_t)v.n * v.dim * sizeof(float), cudaMemcpyHostToDevice, ix->stream)); /* ordered before the normalisation */
     CK(cudaStreamSynchronize(ix->stream));
-    if (v.distance_type == DANN_COSINE) {
-        int blocks = std::min<long long>((v.n + 255) / 256, (long long)ix->sm_count * 8);
-        dann_normalize_rows_kernel<<<std::max(blocks, 1), 256, 0, ix->stream>>>(d, v.n, v.dim);
-        ix->launches++;
-        CK(cudaGetLastError());
-        CK(cudaStreamSynchronize(ix->stream));
-    }
-    return DANN_OK;
+    return normalize_rows(ix, d);
 } DANN_CATCH
 
 extern "C" int dann_index_set_vectors_device(dann_index *ix, float *d_vectors) try {
@@ -948,14 +958,7 @@ extern "C" int dann_index_set_vectors_device(dann_index *ix, float *d_vectors) t
     v.vectors = d_vectors; /* borrowed: not in ix->owned */
     ix->hbm_bytes += (uint64_t)v.n * v.dim * sizeof(float);
     CK(order_after_default_stream(ix, ix->stream)); /* the caller's rows: see DANN_DEVICE_INPUT_STREAM */
-    if (v.distance_type == DANN_COSINE) {
-        int blocks = std::min<long long>((v.n + 255) / 256, (long long)ix->sm_count * 8);
-        dann_normalize_rows_kernel<<<std::max(blocks, 1), 256, 0, ix->stream>>>(d_vectors, v.n, v.dim);
-        ix->launches++;
-        CK(cudaGetLastError());
-        CK(cudaStreamSynchronize(ix->stream));
-    }
-    return DANN_OK;
+    return normalize_rows(ix, d_vectors);
 } DANN_CATCH
 
 extern "C" int dann_index_download_nbrs(dann_index *ix, uint32_t *out) try {
@@ -1177,7 +1180,7 @@ extern "C" int dann_scan_begin(dann_index *ix, dann_scan **out) try {
 static void scan_release(dann_scan *sc) {
     DevBuf *bufs[] = {&sc->d_qindex, &sc->d_step, &sc->d_query, &sc->d_qfull, &sc->d_qcodes, &sc->d_labels, &sc->d_label_off, &sc->d_saved,
                       &sc->d_heap_sm, &sc->d_vis, &sc->d_heap_tail, &sc->d_cnode, &sc->d_set, &sc->d_ins, &sc->d_stream,
-                      &sc->d_slen, &sc->d_stats, &sc->d_dist, &sc->d_win, &sc->d_winst, &sc->d_row, &sc->d_ctl};
+                      &sc->d_slen, &sc->d_stats, &sc->d_dist, &sc->d_win, &sc->d_winst, &sc->d_ctl};
     for (DevBuf *b : bufs) b->release();
 }
 
@@ -1226,11 +1229,7 @@ extern "C" int dann_scan_rescan(dann_scan *sc, const float *query, const int16_t
     else sc->query.assign(dim, 0.0f); /* NULL order-by argument: zero vector, no labels (labels/mod.rs:214-216) */
     sc->nlabels = query ? nlabels : -1;
     sc->labels.clear();
-    if (sc->nlabels > 0) { /* LabelSet::from(Vec): sort_unstable + dedup (labels/mod.rs:30-37) */
-        sc->labels.assign(labels, labels + nlabels);
-        std::sort(sc->labels.begin(), sc->labels.end());
-        sc->labels.erase(std::unique(sc->labels.begin(), sc->labels.end()), sc->labels.end());
-    }
+    if (sc->nlabels > 0) append_label_set(sc->labels, labels, labels + nlabels);
     sc->L = search_list_size;
     sc->rescore = rescore;
     sc->grow = 1;
@@ -1245,7 +1244,7 @@ extern "C" int dann_scan_rescan(dann_scan *sc, const float *query, const int16_t
     CK(sc->d_stats.reserve(sizeof(dann_query_stats)));
     CK(sc->d_win.reserve((size_t)std::max(rescore, 1) * 8));
     CK(sc->d_winst.reserve(sizeof(ScanWindow)));
-    CK(sc->d_row.reserve(sizeof(ScanRow)));
+    CK(sc->d_step.reserve(sizeof(ScanStepOut)));
     CK(sc->d_ctl.reserve(64));
     CK(cudaMemcpyAsync(sc->d_query.p, sc->query.data(), (size_t)dim * 4, cudaMemcpyHostToDevice, st));
     if (sc->nlabels >= 0) {
@@ -1256,16 +1255,10 @@ extern "C" int dann_scan_rescan(dann_scan *sc, const float *query, const int16_t
         CK(cudaMemcpyAsync(sc->d_label_off.p, off, 8, cudaMemcpyHostToDevice, st));
     }
     CK(cudaMemsetAsync(sc->d_winst.p, 0, sizeof(ScanWindow), st));
-    if (ix->plain) {
-        CK(sc->d_qindex.reserve((size_t)v.dim_index * 4));
-        dann_prepare_plain_kernel<<<1, 128, 0, st>>>(v.dim, v.dim_index, v.distance_type == DANN_COSINE, sc->d_query.as<float>(),
-                                                    sc->d_qfull.as<float>(), sc->d_qindex.as<float>());
-        ix->launches++;
-        CK(cudaGetLastError());
-    } else {
-        rc = launch_prepare(ix, sc->d_query.as<float>(), 1, sc->d_qfull.as<float>(), sc->d_qcodes.as<uint64_t>(), st);
-        if (rc) return rc;
-    }
+    if (ix->plain) CK(sc->d_qindex.reserve((size_t)v.dim_index * 4));
+    rc = launch_prepare(ix, sc->d_query.as<float>(), 1, sc->d_qfull.as<float>(), sc->d_qcodes.as<uint64_t>(),
+                        sc->d_qindex.as<float>(), st);
+    if (rc) return rc;
     rc = scan_reset_search(sc);
     if (rc) return rc;
     CK(cudaStreamSynchronize(st));
@@ -1315,62 +1308,32 @@ static int scan_launch_search(dann_scan *sc, uint32_t want) {
     return DANN_OK;
 }
 
-/* Pull `need` more rows off the approximate stream into d_stream[skip ..]; returns how many came. */
-static int scan_pull(dann_scan *sc, uint32_t need, uint32_t *got, uint32_t *skip_out) {
+/* next_with_resort (scan.rs:244-305): `while resort_buffer.len() < resort_size { next() ... }` then pop; with
+ * resort_size == 0 it is a plain next().  The search, the exact distances of the rows it appended and the window step
+ * are enqueued back to back (see dann_scan_finish_kernel) and one ScanStepOut comes back: one host synchronisation. */
+extern "C" int dann_scan_gettuple(dann_scan *sc, uint32_t *block, uint16_t *offset, uint32_t *node_id, float *dist) try {
+    if (!sc) return fail(DANN_ERR_INVALID_ARG, "dann_scan_gettuple: NULL scan");
+    if (!sc->active) return fail(DANN_ERR_STATE, "dann_scan_gettuple before dann_scan_rescan");
     dann_index *ix = sc->ix;
-    cudaStream_t st = ix->stream;
-    uint32_t skip = 0; /* rows that are only re-generated because the workspace had to grow */
-    for (int attempt = 0;; attempt++) {
-        const uint32_t want = skip + need;
-        int lrc = scan_launch_search(sc, want);
-        if (lrc) return lrc;
-        uint32_t *d_ctl = sc->d_ctl.as<uint32_t>();
-        struct {
-            uint32_t ctl[2];
-        } h;
-        CK(cudaMemcpyAsync(h.ctl, d_ctl, 8, cudaMemcpyDeviceToHost, st));
-        uint32_t slen = 0;
-        CK(cudaMemcpyAsync(&slen, sc->d_slen.p, 4, cudaMemcpyDeviceToHost, st));
-        CK(cudaMemcpyAsync(&sc->stats, sc->d_stats.p, sizeof(dann_query_stats), cudaMemcpyDeviceToHost, st));
-        CK(cudaStreamSynchronize(st));
-        if (h.ctl[1] == 0) {
-            if (slen < want) sc->exhausted = true;
-            *got = slen > skip ? slen - skip : 0;
-            *skip_out = skip;
-            return DANN_OK;
-        }
-        /* the scan outgrew its workspace: rebuild it twice as large and replay the stream up to here */
-        if (attempt >= 8) return fail(DANN_ERR_CAPACITY, "scan workspace still too small after %d growth steps", attempt);
-        sc->grow *= 2;
-        int rc = scan_reset_search(sc);
-        if (rc) return rc;
-        skip = sc->streamed;
-    }
-}
-
-/* DANN_SCAN_FUSED=1: the same amgettuple with ONE host synchronisation: search, exact distances of the new rows and the
- * window step are enqueued back to back (the kernels read the search's outcome from device memory) and a single
- * ScanStepOut comes back.  Same rows, same counters after every call; opt-in until it has been timed on hardware. */
-static int gettuple_fused(dann_scan *sc, uint32_t *block, uint16_t *offset, uint32_t *node_id, float *dist) {
-    dann_index *ix = sc->ix;
+    int rc = check_live(ix);
+    if (rc) return rc;
+    std::lock_guard<std::mutex> lk(ix->mu);
     const IndexView &v = ix->v;
     cudaStream_t st = ix->stream;
     const uint32_t rescore = (uint32_t)sc->rescore;
     const uint32_t need = rescore == 0 ? 1u : (sc->win_len < rescore ? rescore - sc->win_len : 0u);
     const bool searching = need && !sc->exhausted;
-    CK(sc->d_step.reserve(sizeof(ScanStepOut)));
     ScanStepOut o;
-    uint32_t skip = 0;
+    uint32_t skip = 0; /* rows that are only re-generated because the workspace had to grow */
     for (int attempt = 0;; attempt++) {
         const uint32_t want = skip + need;
         if (searching) {
-            int lrc = scan_launch_search(sc, want);
-            if (lrc) return lrc;
+            rc = scan_launch_search(sc, want);
+            if (rc) return rc;
             if (rescore > 0) {
                 CK(sc->d_dist.reserve((size_t)want * 4));
                 size_t smem = (size_t)((v.dim + 3u) & ~3u) * sizeof(float) + DANN_SMEM_SLACK;
-                if (smem > 48 * 1024)
-                    CK(cudaFuncSetAttribute(dann_scan_distance_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+                CK(allow_dynamic_smem(dann_scan_distance_kernel, smem));
                 dann_scan_distance_kernel<<<1, 128, smem, st>>>(v, sc->d_qfull.as<float>(), sc->d_stream.as<uint32_t>(),
                                                                sc->d_slen.as<uint32_t>(), sc->d_ctl.as<uint32_t>() + 1, skip,
                                                                sc->d_dist.as<float>());
@@ -1398,13 +1361,13 @@ static int gettuple_fused(dann_scan *sc, uint32_t *block, uint16_t *offset, uint
         /* the scan outgrew its workspace: rebuild it twice as large and replay the stream up to here */
         if (attempt >= 8) return fail(DANN_ERR_CAPACITY, "scan workspace still too small after %d growth steps", attempt);
         sc->grow *= 2;
-        int rrc = scan_reset_search(sc);
-        if (rrc) return rrc;
+        rc = scan_reset_search(sc);
+        if (rc) return rc;
         skip = sc->streamed;
     }
     sc->win_len = o.win.len;
     sc->stats.d_full = o.win.d_full;
-    if (ix->plain) {
+    if (ix->plain) { /* every comparison of the beam search was a full-distance comparison (plain/storage.rs:238,288) */
         sc->stats.d_full += sc->stats.candidates;
         sc->stats.d_quantized = 0;
     }
@@ -1414,63 +1377,6 @@ static int gettuple_fused(dann_scan *sc, uint32_t *block, uint16_t *offset, uint
     if (offset) *offset = (uint16_t)(o.row.tid & 0xFFFFu);
     if (node_id) *node_id = o.row.node;
     if (dist) *dist = o.row.dist;
-    return 1;
-}
-
-extern "C" int dann_scan_gettuple(dann_scan *sc, uint32_t *block, uint16_t *offset, uint32_t *node_id, float *dist) try {
-    if (!sc) return fail(DANN_ERR_INVALID_ARG, "dann_scan_gettuple: NULL scan");
-    if (!sc->active) return fail(DANN_ERR_STATE, "dann_scan_gettuple before dann_scan_rescan");
-    dann_index *ix = sc->ix;
-    int rc = check_live(ix);
-    if (rc) return rc;
-    std::lock_guard<std::mutex> lk(ix->mu);
-    /* one host synchronisation per row is the default (the step-by-step path waits for the host between its kernels;
-     * bench.py --mode scan times both); DANN_SCAN_FUSED=0 selects the step-by-step path below */
-    if (env_u32("DANN_SCAN_FUSED", 1) == 1) return gettuple_fused(sc, block, offset, node_id, dist);
-    const IndexView &v = ix->v;
-    cudaStream_t st = ix->stream;
-    /* next_with_resort (scan.rs:244-305): `while resort_buffer.len() < resort_size { next() ... }` then pop;
-     * with resort_size == 0 it is a plain next() */
-    const uint32_t rescore = (uint32_t)sc->rescore;
-    uint32_t need = rescore == 0 ? 1u : (sc->win_len < rescore ? rescore - sc->win_len : 0u);
-    uint32_t got = 0, skip = 0;
-    if (need && !sc->exhausted) {
-        rc = scan_pull(sc, need, &got, &skip);
-        if (rc) return rc;
-        sc->streamed += got;
-    }
-    if (rescore > 0 && got > 0) { /* get_full_distance_for_resort for the rows that just arrived */
-        CK(sc->d_dist.reserve((size_t)(skip + got) * 4));
-        size_t smem = (size_t)((v.dim + 3u) & ~3u) * sizeof(float) + DANN_SMEM_SLACK;
-        if (smem > 48 * 1024)
-            CK(cudaFuncSetAttribute(dann_full_distance_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        dann_full_distance_kernel<<<1, 128, smem, st>>>(v, sc->d_qfull.as<float>(), sc->d_stream.as<uint32_t>(),
-                                                       (int)(skip + got), sc->d_dist.as<float>());
-        ix->launches++;
-        CK(cudaGetLastError());
-    }
-    dann_scan_resort_kernel<<<1, 32, 0, st>>>(v, sc->d_winst.as<ScanWindow>(), sc->d_win.as<uint64_t>(), rescore,
-                                             sc->d_stream.as<uint32_t>(), sc->d_dist.as<float>(), skip, skip + got,
-                                             sc->d_row.as<ScanRow>());
-    ix->launches++;
-    CK(cudaGetLastError());
-    ScanRow row;
-    ScanWindow ws;
-    CK(cudaMemcpyAsync(&row, sc->d_row.p, sizeof(ScanRow), cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(&ws, sc->d_winst.p, sizeof(ScanWindow), cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
-    sc->win_len = ws.len;
-    sc->stats.d_full = ws.d_full;
-    if (ix->plain) { /* every comparison of the beam search was a full-distance comparison (plain/storage.rs:238,288) */
-        sc->stats.d_full += sc->stats.candidates;
-        sc->stats.d_quantized = 0;
-    }
-    sc->stats.stream_len = sc->streamed;
-    if (!row.have) return 0;
-    if (block) *block = (uint32_t)(row.tid >> 16);
-    if (offset) *offset = (uint16_t)(row.tid & 0xFFFFu);
-    if (node_id) *node_id = row.node;
-    if (dist) *dist = row.dist;
     return 1;
 } DANN_CATCH
 

@@ -84,17 +84,16 @@ def test_address_sanitizer_finds_nothing_in_host_code_or_kernels():
     assert passed == 80 + 12
     passed, _ = _run(["tests/test_zz_f_fuzz_gpu.py"],
                      {"DANN_FUZZ_SEEDS": "80", "DANN_SEARCH_KERNEL": "3", "DANN_SEARCH_HS": "16", "DANN_DEBUG_SHRINK": "8",
-                      "DANN_SCAN_FUSED": "1", "SIMT_SCHED": "2", "SIMT_SM_COUNT": "2"}, asan=True)
+                      "SIMT_SCHED": "2", "SIMT_SM_COUNT": "2"}, asan=True)
     assert passed == 80 + 12
 
 
-def test_one_synchronisation_gettuple_passes_under_emulation():
-    """amgettuple with a single host synchronisation per row is the default (DANN_SCAN_FUSED=1); the step-by-step path
-    (DANN_SCAN_FUSED=0) stays covered here."""
-    passed, _ = _run(["tests/test_gpu_parity.py", "-k", "scan or gettuple or counters or null or empty"],
-                     {"DANN_SCAN_FUSED": "0"})
+def test_scan_operator_under_forced_workspace_growth_passes_under_emulation():
+    """The scan operator's tests, then edge-case fuzz with every first workspace too small: amgettuple regrows the
+    suspended search and replays the stream, under the default lane schedule."""
+    passed, _ = _run(["tests/test_gpu_parity.py", "-k", "scan or gettuple or counters or null or empty"])
     assert passed >= 2
-    passed, _ = _run(["tests/test_zz_f_fuzz_gpu.py"], {"DANN_SCAN_FUSED": "0", "DANN_DEBUG_SHRINK": "8", "DANN_FUZZ_SEEDS": "120"})
+    passed, _ = _run(["tests/test_zz_f_fuzz_gpu.py"], {"DANN_DEBUG_SHRINK": "8", "DANN_FUZZ_SEEDS": "120"})
     assert passed == 120 + 12     # the seeds + the four reference-KAT cases and the eight medium cases in the same file
 
 

@@ -1,7 +1,6 @@
 """GPU parity of the plain (uncompressed) storage layout - SURVEY.md §8f row 3: plain/storage.rs:223-307,
-scan.rs:392-403 - and of the one-synchronisation amgettuple (DANN_SCAN_FUSED=1), through the C ABI: batch calls, the
-streaming scan operator with counters after every row, golden vectors, edge-case fuzz.  Part of the regular
-`-m gpu` run."""
+scan.rs:392-403 - and of the one-synchronisation amgettuple, through the C ABI: batch calls, the streaming scan
+operator with counters after every row, golden vectors, edge-case fuzz.  Part of the regular `-m gpu` run."""
 import os
 
 import numpy as np
@@ -121,14 +120,12 @@ def test_plain_storage_random_small_indexes(lib, monkeypatch, seed):
         sc.end()
 
 
-@pytest.mark.parametrize("fused", ["1", "0"])
-def test_one_synchronisation_gettuple_and_the_step_by_step_path_stream_alike(lib, monkeypatch, fused):
-    """DANN_SCAN_FUSED=1 (default: dann_scan_distance_kernel / dann_scan_finish_kernel, one synchronisation per row) and
-    DANN_SCAN_FUSED=0 (step by step): same rows and counters after every call."""
+def test_one_synchronisation_gettuple_rows_and_counters_match_oracle(lib):
+    """amgettuple (dann_scan_distance_kernel / dann_scan_finish_kernel, one synchronisation per row): the row and all
+    four counters equal oracle.scan's after every call, across rescans with and without a window and a label key."""
     from oracle import oracle
     s = build_case(3000, 128, COSINE, seed=21, kind="normal", labels=True, deleted_every=9)
     q = _queries(s, 4, 3)
-    monkeypatch.setenv("DANN_SCAN_FUSED", fused)
     with lib.DiskAnnIndex(s) as idx:
         sc = idx.begin_scan()
         for qi, (L, rescore, key) in enumerate(((40, 10, None), (25, 0, None), (60, 50, [3, 9]), (30, 5, None))):

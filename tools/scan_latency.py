@@ -1,8 +1,7 @@
 """bench.py --mode scan: latency of the OPERATOR SURFACE the reference exposes - one backend, one scan at a time:
 amrescan + k x amgettuple (scan.rs:336-405) through dann_scan_rescan / dann_scan_gettuple - next to the CPU oracle
-doing the same single-threaded (BASELINE.md §3 "CPU-1: p50/p95").  The default amgettuple makes one host
-synchronisation per row; the step-by-step flavour (DANN_SCAN_FUSED=0) is timed beside it.  bench.py's default run
-calls measure() on the loaded 20M index and attaches the result as "operator".
+doing the same single-threaded (BASELINE.md §3 "CPU-1: p50/p95").  amgettuple makes one host synchronisation per row.
+bench.py's default run calls measure() on the loaded 20M index and attaches the result as "operator".
 
 The index is the bench fixture (default here: configs[1], 1M x 768; pass --n for larger).  One JSON line."""
 from __future__ import annotations
@@ -18,14 +17,13 @@ def _pct(v, p):
     return round(v[min(len(v) - 1, int(len(v) * p))], 4)
 
 
-def measure(idx, snap, oracle, q, L, rescore, k, warm=20, both=True):
+# `both` is unused; bench.py passes both=False
+def measure(idx, snap, oracle, q, L, rescore, k, warm=20, both=False):
     """amrescan + k x amgettuple, one scan at a time, for every row of q (host array; the heap rows the oracle reranks for
-    these queries must already be resident in snap.vectors) -> dict.  `both`: also time DANN_SCAN_FUSED=0 (one launch
-    and one synchronisation per step instead of one synchronisation per row)."""
+    these queries must already be resident in snap.vectors) -> dict."""
     nq = q.shape[0]
 
-    def one_pass(fused):
-        os.environ["DANN_SCAN_FUSED"] = "1" if fused else "0"
+    def one_pass():
         sc = idx.begin_scan()
         first, per_row, whole, got = [], [], [], []
         for i in range(nq):
@@ -43,14 +41,12 @@ def measure(idx, snap, oracle, q, L, rescore, k, warm=20, both=True):
                 whole.append((t2 - t0) * 1e3)
             got.append([(x[0] << 16) | x[1] if x else 0xFFFFFFFFFFFFFFFF for x in out])
         sc.end()
-        os.environ.pop("DANN_SCAN_FUSED", None)
         return {"rescan_plus_first_row_ms": {"p50": _pct(first, 0.5), "p95": _pct(first, 0.95)},
                 "next_row_ms": {"p50": _pct(per_row, 0.5), "p95": _pct(per_row, 0.95)},
                 "scan_of_k_rows_ms": {"p50": _pct(whole, 0.5), "p95": _pct(whole, 0.95)},
                 "scans_per_s_one_backend": round(1e3 / (sum(whole) / len(whole)), 1)}, np.array(got, dtype=np.uint64)
 
-    res_fused, tids_f = one_pass(True)
-    res_steps, tids_s = one_pass(False) if both else (None, None)
+    res, tids = one_pass()
     # CPU: the oracle, one query at a time on one thread (= one Postgres backend)
     lat = []
     otid = np.zeros((nq, k), np.uint64)
@@ -61,13 +57,10 @@ def measure(idx, snap, oracle, q, L, rescore, k, warm=20, both=True):
             lat.append((time.perf_counter() - t0) * 1e3)
         otid[i] = t[0]
     out = {"scans": nq - warm, "search_list_size": L, "rescore": rescore, "k": k,
-           "gettuple": res_fused,
+           "gettuple": res,
            "cpu_oracle_single_thread_ms": {"p50": _pct(lat, 0.5), "p95": _pct(lat, 0.95),
                                            "scans_per_s_one_backend": round(1e3 / (sum(lat) / len(lat)), 1)},
-           "parity": {"rows_identical": bool(np.array_equal(tids_f, otid))}}
-    if both:
-        out["gettuple_step_by_step (DANN_SCAN_FUSED=0)"] = res_steps
-        out["parity"]["step_by_step_rows_identical"] = bool(np.array_equal(tids_s, otid))
+           "parity": {"rows_identical": bool(np.array_equal(tids, otid))}}
     return out
 
 
