@@ -30,11 +30,37 @@
 /* ------------------------------------------------------------------------------------ */
 #define DANN_SMEM_SLACK 128u /* bytes behind every dynamic shared-memory window (see launch_prepare) */
 
-/* A launch gets at most 48 KB of dynamic shared memory unless its kernel has opted in to more. */
+/* The static __shared__ bytes of `kernel`: they come off the shared memory a launch of it may take.  The CPU emulator
+ * (tests/simt) keeps static shared variables outside the simulated window, so there they take none. */
+template <typename K>
+static cudaError_t static_smem_bytes(K kernel, size_t *bytes) {
+#ifdef DANN_SIMT_EMU
+    (void)kernel;
+    *bytes = 0;
+    return cudaSuccess;
+#else
+    cudaFuncAttributes fa;
+    const cudaError_t e = cudaFuncGetAttributes(&fa, kernel);
+    *bytes = e == cudaSuccess ? fa.sharedSizeBytes : 0;
+    return e;
+#endif
+}
+
+/* A launch gets at most 48 KB of shared memory, the kernel's static __shared__ included, unless its kernel has opted in
+ * to more.  (A 12256-d query row fills a 48 KB window exactly; with the few static bytes of the staging kernels, such as
+ * the mbarrier of stage_query_row, it needs the opt-in.) */
 template <typename K>
 static cudaError_t allow_dynamic_smem(K kernel, size_t bytes) {
-    if (bytes <= 48 * 1024) return cudaSuccess;
+    size_t fixed = 0;
+    const cudaError_t e = static_smem_bytes(kernel, &fixed);
+    if (e != cudaSuccess || bytes + fixed <= 48 * 1024) return e;
     return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
+}
+
+/* dynamic shared memory of one dann_rerank_kernel CTA (its layout is in dann_kernels.cuh): the query row, one f32 per
+ * streamed row rounded up to an even count, the rescore window of 8-byte entries, 16 bytes, DANN_SMEM_SLACK */
+static size_t rerank_smem_bytes(uint32_t dim, uint32_t c_target, uint32_t rescore) {
+    return (size_t)((dim + 3u) & ~3u) * 4 + (size_t)((c_target + 1u) & ~1u) * 4 + (size_t)rescore * 8 + 16 + DANN_SMEM_SLACK;
 }
 
 /* LabelSet::from(Vec): sort_unstable + dedup (labels/mod.rs:30-37) of [first, last), appended to `out` */
@@ -131,6 +157,7 @@ struct dann_index {
     std::mutex mu;
     int sm_count = 0;
     size_t smem_optin = 0;
+    size_t rerank_smem_max = 0; /* dynamic shared memory a dann_rerank_kernel launch may take: smem_optin less its static */
     std::atomic<uint64_t> launches{0}; /* bumped by entry points that do not take `mu` too */
     bool poisoned = false;
     /* per-warp-slot search workspace */
@@ -348,6 +375,9 @@ static int index_load_impl(const dann_snapshot_desc *s, const float *index_vecto
     CK(cudaGetDeviceProperties(&prop, device));
     ix->sm_count = prop.multiProcessorCount;
     ix->smem_optin = prop.sharedMemPerBlockOptin;
+    size_t rerank_static = 0;
+    CK(static_smem_bytes(dann_rerank_kernel, &rerank_static));
+    ix->rerank_smem_max = ix->smem_optin > rerank_static ? ix->smem_optin - rerank_static : 0;
     CK(cudaStreamCreateWithFlags(&ix->stream, cudaStreamNonBlocking));
     for (auto &e : ix->ev) CK(cudaEventCreate(&e));
     CK(cudaEventCreateWithFlags(&ix->ev_order, cudaEventDisableTiming));
@@ -768,12 +798,6 @@ static int search_batch_device_locked(dann_index *ix, const float *d_queries, co
     if (L < 1 || L > 10000) return fail(DANN_ERR_INVALID_ARG, "search_list_size %d outside 1..10000 (guc.rs:11-26)", L);
     if (rescore < 0 || rescore > 1000) return fail(DANN_ERR_INVALID_ARG, "rescore %d outside 0..1000 (guc.rs:28-43)", rescore);
     if (!d_queries || !d_out_tid) return fail(DANN_ERR_INVALID_ARG, "NULL query or output buffer");
-    {   /* the rerank kernel keeps one f32 per streamed row + the window in shared memory */
-        const size_t need_smem = (size_t)((v.dim + 3u) & ~3u) * 4 + ((size_t)rescore + (size_t)k + 2) * 4 + (size_t)rescore * 8 + 64;
-        if (need_smem > ix->smem_optin)
-            return fail(DANN_ERR_INVALID_ARG, "k=%d rows with rescore=%d need %zu B of shared memory per scan (limit %zu): "
-                        "fetch fewer rows per scan", k, rescore, need_smem, ix->smem_optin);
-    }
     if (ix->plain) {
         if (d_label_off) return fail(DANN_ERR_INVALID_ARG, "plain storage does not support label filters (plain/storage.rs:260)");
         /* scan.rs:392-403: a plain index only resorts when it holds fewer dimensions than the heap column */
@@ -782,6 +806,12 @@ static int search_batch_device_locked(dann_index *ix, const float *d_queries, co
     if (rescore > 0 && v.n && !v.vectors) return fail(DANN_ERR_STATE, "index has no heap vectors yet (dann_index_set_vectors): rescore must be 0");
     /* rows needed from the approximate stream: scan.rs:255-305 */
     const uint32_t c_target = rescore == 0 ? (uint32_t)k : (uint32_t)rescore + (uint32_t)k - 1u;
+    /* the rerank kernel keeps the query row, one f32 per streamed row and the window in shared memory; a request past
+     * the limit is refused here, because a failed launch would poison the handle */
+    const size_t rerank_smem = rerank_smem_bytes(v.dim, c_target, (uint32_t)rescore);
+    if (rerank_smem > ix->rerank_smem_max)
+        return fail(DANN_ERR_INVALID_ARG, "k=%d rows with rescore=%d need %zu B of shared memory per scan (limit %zu): "
+                    "fetch fewer rows per scan", k, rescore, rerank_smem, ix->rerank_smem_max);
 
     CK(ix->sc_qfull.reserve((size_t)B * v.dim * sizeof(float)));
     CK(ix->sc_qcodes.reserve((size_t)B * v.cw * sizeof(uint64_t)));
@@ -818,9 +848,8 @@ static int search_batch_device_locked(dann_index *ix, const float *d_queries, co
     r.out_node = d_out_node;
     r.out_count = d_out_count;
     r.stats = d_stats;
-    size_t smem = (size_t)((v.dim + 3u) & ~3u) * 4 + (size_t)((c_target + 1u) & ~1u) * 4 + (size_t)rescore * 8 + 16 + DANN_SMEM_SLACK;
-    CK(allow_dynamic_smem(dann_rerank_kernel, smem));
-    dann_rerank_kernel<<<B, 128, smem, st>>>(r);
+    CK(allow_dynamic_smem(dann_rerank_kernel, rerank_smem));
+    dann_rerank_kernel<<<B, 128, rerank_smem, st>>>(r);
     ix->launches++;
     CK(cudaGetLastError());
     if (ix->plain && rescore > 0) {

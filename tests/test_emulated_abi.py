@@ -73,6 +73,15 @@ def test_lean_kernel_instantiations_pass_under_emulation():
     assert passed == 25 and "skipped" not in out.splitlines()[-1], out[-500:]
 
 
+def test_wide_codes_and_wide_rows_pass_under_emulation():
+    """tests/test_zz_m_wide_gpu.py, whole: both round-1 search kernels at every code width up to 16000 x 2 bits, the
+    streaming scan (drained through the switch to Ent64), the exact-distance kernels past 48 KB of shared memory, the
+    rerank shared-memory bound and every SBQ-distance instantiation.  None is left out: the slowest case takes about
+    15 s of CPU time."""
+    passed, out = _run(["tests/test_zz_m_wide_gpu.py"], {"SIMT_SCHED": "2"})
+    assert passed == 38 and "skipped" not in out.splitlines()[-1], out[-500:]
+
+
 def test_address_sanitizer_finds_nothing_in_host_code_or_kernels():
     """The emulated ABI built with -fsanitize=address: every "device" buffer is a red-zoned host allocation, so an
     out-of-bounds access by a kernel (or by the host code around it) aborts the run.  Edge-case fuzz with the measured
