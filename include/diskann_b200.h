@@ -136,6 +136,20 @@ int dann_scan_rescan(dann_scan *sc, const float *query, const int16_t *labels, i
  * dist is the exact rerank distance (NaN when rescore == 0). Any output may be NULL. */
 int dann_scan_gettuple(dann_scan *sc, uint32_t *block, uint16_t *offset, uint32_t *node_id,
                        float *dist);
+/* n amgettuple calls, one per scan, all on the same index: out_rc[i] = 1 (row), 0 (end of scan) or a negative status
+ * for that scan alone; block/offset/node_id/dist are [n] arrays, each may be NULL.
+ * Every scan gets exactly the row, dist bits and dann_scan_stats the same sequence of dann_scan_gettuple calls would
+ * give it; the scans may differ in query, key, search_list_size and rescore, and a scan may switch between the two
+ * entry points at any call.  Many suspended searches resume in one kernel launch (one warp each, with the scan's own
+ * plan and workspace), so the backends of a serving process share the GPU instead of queueing behind each other.
+ * Returns DANN_OK, or before anything runs: DANN_ERR_INVALID_ARG for n outside 1..65536, a NULL scans / out_rc / scan,
+ * scans of different indexes or a scan listed twice, DANN_ERR_STATE for a scan that has not been rescanned.  A scan
+ * whose workspace cannot grow further gets DANN_ERR_CAPACITY in out_rc and leaves the others unaffected; so does one
+ * whose buffers cannot be allocated (DANN_ERR_OOM).  Any other failure returns an error only while no scan has taken
+ * its step; once one has, it goes to out_rc of the scans it hit, and the rows of the others stand.  dann_last_error()
+ * describes the last failure of the call, which need not be scan i's. */
+int dann_scan_gettuple_many(dann_scan *const *scans, int n, int32_t *out_rc, uint32_t *block, uint16_t *offset,
+                            uint32_t *node_id, float *dist);
 int dann_scan_stats(dann_scan *sc, dann_query_stats *out);
 void dann_scan_end(dann_scan *sc);
 
@@ -335,6 +349,16 @@ int dann_coalescer_create(dann_index *ix, int max_batch, int max_wait_us, dann_c
 int dann_coalescer_search(dann_coalescer *c, const float *query, const int16_t *labels, int nlabels, int k,
                           int search_list_size, int rescore, uint64_t *out_tid, float *out_dist,
                           uint32_t *out_count, dann_query_stats *out_stats);
+/* One amgettuple of `sc`, a scan of the coalescer's index: blocks and returns exactly what dann_scan_gettuple would
+ * (1 row, 0 end of scan, < 0 error).  The gettuple calls that arrive within max_wait_us of each other (at most
+ * max_batch, any search_list_size / rescore / key) become one dann_scan_gettuple_many; search and gettuple calls never
+ * share one.  A scan stays single-threaded: at most one call on it at a time; a second call on a scan that already
+ * has one in the same dispatch is refused alone (DANN_ERR_INVALID_ARG) and the other callers are unaffected.  The
+ * message of a failed call is that of its own scan. */
+int dann_coalescer_gettuple(dann_coalescer *c, dann_scan *sc, uint32_t *block, uint16_t *offset, uint32_t *node_id,
+                            float *dist);
+/* batches / queries / largest_batch count the dispatches of both kinds: one dann_search_batch or one
+ * dann_scan_gettuple_many is one batch, each search or gettuple request one query. */
 int dann_coalescer_stats(dann_coalescer *c, uint64_t *batches, uint64_t *queries, uint64_t *largest_batch);
 void dann_coalescer_destroy(dann_coalescer *c); /* drains what is queued, then stops; destroy before dann_index_free */
 

@@ -6,7 +6,10 @@
 // of host threads (one per connected backend) submit single queries and block; a dispatcher thread gathers what
 // arrives within a short window into ONE dann_search_batch call and hands every caller its own rows.  Queries are
 // independent units, so each caller gets exactly what a private scan would have returned.
-// Included at the end of diskann_b200.cu (it uses search_batch_host and fail()); pure host code.
+// The same dispatcher coalesces amgettuple calls: the gettuple requests of a window (any scans of the index, whatever
+// their search_list_size, rescore or key) become ONE dann_scan_gettuple_many call, and each caller gets the row its
+// own dann_scan_gettuple would have returned.  Search and gettuple requests never share a dispatch.
+// Included at the end of diskann_b200.cu (it uses search_batch_host, scan_gettuple_many and fail()); pure host code.
 #pragma once
 #include <chrono>
 #include <condition_variable>
@@ -22,6 +25,13 @@ struct CoalescedRequest {
     float *out_dist;
     uint32_t *out_count;
     dann_query_stats *out_stats;
+    /* gettuple request (scan != NULL): one amgettuple of `scan`, outputs as dann_scan_gettuple's */
+    dann_scan *scan = nullptr;
+    uint32_t *block = nullptr;
+    uint16_t *offset = nullptr;
+    uint32_t *node_id = nullptr;
+    float *dist = nullptr;
+    int row = 0; /* 1 row, 0 end of scan */
     int rc = 0;
     bool done = false;
     std::string err;
@@ -40,6 +50,8 @@ struct dann_coalescer {
     uint64_t n_batches = 0, n_queries = 0, max_seen = 0;
 
     static bool compatible(const CoalescedRequest *a, const CoalescedRequest *b) {
+        /* gettuple requests all go into one dann_scan_gettuple_many call */
+        if (a->scan || b->scan) return a->scan && b->scan;
         /* one dann_search_batch call shares k / L / rescore and is either all keyed or all unkeyed */
         return a->k == b->k && a->L == b->L && a->rescore == b->rescore && (a->nlabels >= 0) == (b->nlabels >= 0);
     }
@@ -102,6 +114,7 @@ struct dann_coalescer {
     }
 
     void execute(std::vector<CoalescedRequest *> &batch) {
+        if (batch[0]->scan) return execute_gettuple(batch);
         const int B = (int)batch.size();
         const uint32_t dim = ix->v.dim;
         const int k = batch[0]->k;
@@ -137,6 +150,74 @@ struct dann_coalescer {
             if (r->out_stats) *r->out_stats = stats[b];
         }
     }
+
+    void execute_gettuple(std::vector<CoalescedRequest *> &batch) {
+        /* a scan is single-threaded: a second call on a scan that already has one in this dispatch breaks that, and is
+         * refused alone (the first call, and everyone else's, go ahead) */
+        std::vector<std::pair<dann_scan *, int>> order(batch.size());
+        for (size_t i = 0; i < batch.size(); i++) order[i] = {batch[i]->scan, (int)i};
+        std::sort(order.begin(), order.end(), [](const std::pair<dann_scan *, int> &a, const std::pair<dann_scan *, int> &b) {
+            return std::less<dann_scan *>()(a.first, b.first) || (a.first == b.first && a.second < b.second);
+        });
+        std::vector<char> dup(batch.size(), 0);
+        for (size_t j = 1; j < order.size(); j++)
+            if (order[j].first == order[j - 1].first) dup[order[j].second] = 1;
+        std::vector<CoalescedRequest *> run;
+        run.reserve(batch.size());
+        for (size_t i = 0; i < batch.size(); i++) {
+            if (!dup[i]) {
+                run.push_back(batch[i]);
+                continue;
+            }
+            batch[i]->rc = DANN_ERR_INVALID_ARG;
+            batch[i]->err = "dann_coalescer_gettuple: another call on the same scan is in flight (a scan is single-threaded)";
+        }
+        const int n = (int)run.size();
+        std::vector<dann_scan *> scans(n);
+        std::vector<int32_t> rcs(n, 0);
+        std::vector<uint32_t> block(n, 0), node(n, 0);
+        std::vector<uint16_t> offset(n, 0);
+        std::vector<float> dist(n, 0.0f);
+        std::vector<std::string> msgs;
+        for (int i = 0; i < n; i++) scans[i] = run[i]->scan;
+        const int rc = scan_gettuple_many(scans.data(), n, rcs.data(), block.data(), offset.data(), node.data(), dist.data(), &msgs);
+        const std::string err = rc ? g_err : std::string(); /* the call's error */
+        for (int i = 0; i < n; i++) {
+            CoalescedRequest *r = run[i];
+            r->rc = rc ? rc : std::min(rcs[i], 0);
+            if (r->rc) {
+                r->err = rc ? err : msgs[i]; /* a scan's own failure: its own message */
+                continue;
+            }
+            r->row = rcs[i];
+            if (!r->row) continue;
+            if (r->block) *r->block = block[i];
+            if (r->offset) *r->offset = offset[i];
+            if (r->node_id) *r->node_id = node[i];
+            if (r->dist) *r->dist = dist[i];
+        }
+    }
+
+    /* queue `r` and block until the dispatcher has answered it */
+    int submit(CoalescedRequest &r) {
+        std::unique_lock<std::mutex> lk(mu);
+        if (stop) return fail(DANN_ERR_STATE, "coalescer is shutting down");
+        /* `callers` keeps dann_coalescer_destroy from deleting the object while this thread still holds (or is about
+         * to re-acquire, inside cv_done.wait) its mutex */
+        struct Leave {
+            dann_coalescer *c;
+            ~Leave() {
+                if (--c->callers == 0) c->cv_idle.notify_all();
+            }
+        };
+        callers++;
+        Leave leave{this}; /* destroyed before lk: runs under the lock */
+        queue.push_back(&r);
+        cv_work.notify_one();
+        cv_done.wait(lk, [&] { return r.done; });
+        if (r.rc) return fail(r.rc, "%s", r.err.c_str());
+        return DANN_OK;
+    }
 };
 
 extern "C" int dann_coalescer_create(dann_index *ix, int max_batch, int max_wait_us, dann_coalescer **out) try {
@@ -168,23 +249,23 @@ extern "C" int dann_coalescer_search(dann_coalescer *c, const float *query, cons
     r.out_dist = out_dist;
     r.out_count = out_count;
     r.out_stats = out_stats;
-    std::unique_lock<std::mutex> lk(c->mu);
-    if (c->stop) return fail(DANN_ERR_STATE, "coalescer is shutting down");
-    /* `callers` keeps dann_coalescer_destroy from deleting the object while this thread still holds (or is about to
-     * re-acquire, inside cv_done.wait) its mutex */
-    struct Leave {
-        dann_coalescer *c;
-        ~Leave() {
-            if (--c->callers == 0) c->cv_idle.notify_all();
-        }
-    };
-    c->callers++;
-    Leave leave{c}; /* destroyed before lk: runs under the lock */
-    c->queue.push_back(&r);
-    c->cv_work.notify_one();
-    c->cv_done.wait(lk, [&] { return r.done; });
-    if (r.rc) return fail(r.rc, "%s", r.err.c_str());
-    return DANN_OK;
+    return c->submit(r);
+} DANN_CATCH
+
+extern "C" int dann_coalescer_gettuple(dann_coalescer *c, dann_scan *sc, uint32_t *block, uint16_t *offset, uint32_t *node_id,
+                                       float *dist) try {
+    if (!c || !sc) return fail(DANN_ERR_INVALID_ARG, "dann_coalescer_gettuple: NULL argument");
+    /* what would fail the whole dispatch is refused here, for this caller alone */
+    if (sc->ix != c->ix) return fail(DANN_ERR_INVALID_ARG, "dann_coalescer_gettuple: the scan belongs to another index");
+    if (!sc->active) return fail(DANN_ERR_STATE, "dann_coalescer_gettuple before dann_scan_rescan");
+    CoalescedRequest r{};
+    r.scan = sc;
+    r.block = block;
+    r.offset = offset;
+    r.node_id = node_id;
+    r.dist = dist;
+    const int rc = c->submit(r);
+    return rc ? rc : r.row;
 } DANN_CATCH
 
 extern "C" int dann_coalescer_stats(dann_coalescer *c, uint64_t *batches, uint64_t *queries, uint64_t *largest_batch) try {

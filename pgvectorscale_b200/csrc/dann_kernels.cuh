@@ -4,6 +4,7 @@
 //   full_distance    : exact f32 L2 / cosine / inner product, AVX2 summation order
 //   rerank           : get_full_distance_for_resort + the sliding rerank window, a batch at a time
 //   scan_distance / scan_finish : the same for the streaming scan, one amgettuple at a time
+//   scan_distance_many / scan_finish_many : one amgettuple of each of many scans per launch
 //   normalize_rows / pad_rows / check_unique : index load helpers
 // Reference paths are relative to pgvectorscale/src/access_method/.
 // Every f32 operation that decides a result is spelled with an explicit-rounding
@@ -453,23 +454,61 @@ struct ScanStepOut {
     ScanWindow win;
 };
 
+/* Exact distances of the rows a scan's search appended past `skip` (none when it overflowed), into out[skip, slen).
+ * qs: the dynamic window, [dim rounded up to 4].  Block-wide. */
+__device__ __forceinline__ void scan_distance_step(const IndexView &ix, float *qs, uint64_t *bar, const float *q_full,
+                                                   const uint32_t *stream, const uint32_t *slen_p,
+                                                   const uint32_t *overflow_p, uint32_t skip, float *out) {
+    if (*overflow_p) return;
+    const uint32_t slen = *slen_p;
+    if (slen <= skip) return;
+    stage_query_row(qs, q_full, ix.dim, bar);
+    full_distances(ix, qs, stream, skip, slen, out);
+}
+
 __global__ void __launch_bounds__(128) dann_scan_distance_kernel(IndexView ix, const float *q_full, const uint32_t *stream,
                                                                  const uint32_t *slen_p, const uint32_t *overflow_p,
                                                                  uint32_t skip, float *out) {
     DANN_DYN_SMEM(dann_smem);
     float *qs = reinterpret_cast<float *>(dann_smem);
     DANN_STATIC_SMEM uint64_t bar;
-    if (*overflow_p) return;
-    const uint32_t slen = *slen_p;
-    if (slen <= skip) return;
-    stage_query_row(qs, q_full, ix.dim, &bar);
-    full_distances(ix, qs, stream, skip, slen, out);
+    scan_distance_step(ix, qs, &bar, q_full, stream, slen_p, overflow_p, skip, out);
 }
 
-__global__ void dann_scan_finish_kernel(IndexView ix, ScanWindow *w, uint64_t *win, uint32_t rescore, const uint32_t *stream,
-                                        const float *dist, uint32_t skip, const uint32_t *slen_p, uint32_t slen_fixed,
-                                        const uint32_t *overflow_p, const dann_query_stats *stats_p, ScanStepOut *out) {
-    if (threadIdx.x != 0 || blockIdx.x != 0) return;
+/* One amgettuple step of many scans (dann_scan_gettuple_many): the arguments dann_scan_distance_kernel and
+ * dann_scan_finish_kernel take, per scan. */
+struct ScanDistanceDesc {
+    const float *q_full;
+    const uint32_t *stream, *slen_p, *overflow_p;
+    float *out;
+    uint32_t skip, pad;
+};
+struct ScanFinishDesc {
+    ScanWindow *w;
+    uint64_t *win;
+    const uint32_t *stream;
+    const float *dist;
+    const uint32_t *slen_p;     /* NULL: the scan did not search this step */
+    const uint32_t *overflow_p; /* NULL: the scan did not search this step */
+    const dann_query_stats *stats_p;
+    uint32_t rescore, skip, slen_fixed, pad;
+};
+
+/* CTA b: the exact distances of scan d[b], which searched with rescore > 0 */
+__global__ void __launch_bounds__(128) dann_scan_distance_many_kernel(IndexView ix, const ScanDistanceDesc *d) {
+    DANN_DYN_SMEM(dann_smem);
+    float *qs = reinterpret_cast<float *>(dann_smem);
+    DANN_STATIC_SMEM uint64_t bar;
+    const ScanDistanceDesc &e = d[blockIdx.x];
+    scan_distance_step(ix, qs, &bar, e.q_full, e.stream, e.slen_p, e.overflow_p, e.skip, e.out);
+}
+
+/* The window step of one scan: next_with_resort's refill with the rows its search appended, then one pop; *out gathers
+ * what the host needs (overflow bits, rows produced, counters, the row, the window) */
+__device__ __forceinline__ void scan_finish_step(const IndexView &ix, ScanWindow *w, uint64_t *win, uint32_t rescore,
+                                                 const uint32_t *stream, const float *dist, uint32_t skip,
+                                                 const uint32_t *slen_p, uint32_t slen_fixed, const uint32_t *overflow_p,
+                                                 const dann_query_stats *stats_p, ScanStepOut *out) {
     ScanStepOut o;
     o.overflow = overflow_p ? *overflow_p : 0u;
     o.slen = slen_p ? *slen_p : slen_fixed; /* no search this call: nothing new beyond `skip` */
@@ -514,5 +553,22 @@ __global__ void dann_scan_finish_kernel(IndexView ix, ScanWindow *w, uint64_t *w
     o.win.len = len;
     o.win.d_full = dfull;
     *out = o;
+}
+
+__global__ void dann_scan_finish_kernel(IndexView ix, ScanWindow *w, uint64_t *win, uint32_t rescore, const uint32_t *stream,
+                                        const float *dist, uint32_t skip, const uint32_t *slen_p, uint32_t slen_fixed,
+                                        const uint32_t *overflow_p, const dann_query_stats *stats_p, ScanStepOut *out) {
+    if (threadIdx.x != 0 || blockIdx.x != 0) return;
+    scan_finish_step(ix, w, win, rescore, stream, dist, skip, slen_p, slen_fixed, overflow_p, stats_p, out);
+}
+
+/* thread i: the window step of scan d[i], its outcome into out[i] (one copy brings every scan's back) */
+__global__ void __launch_bounds__(128) dann_scan_finish_many_kernel(IndexView ix, const ScanFinishDesc *d, uint32_t n,
+                                                                    ScanStepOut *out) {
+    const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const ScanFinishDesc f = d[i];
+    scan_finish_step(ix, f.w, f.win, f.rescore, f.stream, f.dist, f.skip, f.slen_p, f.slen_fixed, f.overflow_p, f.stats_p,
+                     out + i);
 }
 

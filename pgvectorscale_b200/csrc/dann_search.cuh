@@ -427,6 +427,27 @@ struct SearchWarp {
     }
 };
 
+/* The warp's storage: its per_warp_smem layout at `base` (visited list, heap top, staging list, PLAIN query slice) and
+ * workspace slot `slot` of the HBM arrays.  dann_search_kernel below carves the same layout inline: called from there,
+ * this helper changes the order ptxas schedules that kernel in, and its measured SASS is kept as it is. */
+template <typename T, int NCH, int PLAIN>
+__device__ __forceinline__ void bind_search_warp(SearchWarp<T, NCH, PLAIN> &w, const SearchArgs &a, unsigned char *base,
+                                                 uint32_t slot) {
+    using E = typename T::E;
+    w.vis = reinterpret_cast<uint64_t *>(base);
+    E *hsm = reinterpret_cast<E *>(base + (size_t)a.vcap * 8);
+    w.list = reinterpret_cast<uint32_t *>(base + (size_t)a.vcap * 8 + (size_t)a.hs * sizeof(E));
+    w.dl = w.list + DANN_LIST_CAP;
+    w.qrow = reinterpret_cast<float *>(w.dl + DANN_LIST_CAP); /* PLAIN only: [plain_dim rounded up to 4] */
+    w.hash = a.hash + (size_t)slot * a.hash_cap;
+    w.bitmap = a.bitmap + (size_t)slot * a.bitmap_words;
+    w.ins = a.ins_list + (size_t)slot * a.ins_cap;
+    w.cnode = a.cand_node + (size_t)slot * a.cand_cap;
+    w.heap.sm = hsm;
+    w.heap.gl = reinterpret_cast<E *>(a.heap_tail) + (size_t)slot * a.cand_cap;
+    w.heap.hs = a.hs;
+}
+
 template <typename T, int NCH, int PLAIN = 0>
 __global__ void __launch_bounds__(384, 1) dann_search_kernel(const SearchArgs a) {
     using E = typename T::E;
@@ -448,4 +469,31 @@ __global__ void __launch_bounds__(384, 1) dann_search_kernel(const SearchArgs a)
     w.heap.gl = reinterpret_cast<E *>(a.heap_tail) + (size_t)slot * a.cand_cap;
     w.heap.hs = a.hs;
     serve_queries(a, lane, w);
+}
+
+/* Many suspended scans in one launch (dann_scan_gettuple_many): CTA b is one warp that resumes scan b for one amgettuple
+ * step.  args[b] is that scan's own launch (nq = 1, its saved state, its private workspace, its c_target and plan), so
+ * the scans of one launch may differ in everything but the instantiation.  The arguments are copied into shared memory
+ * first, so that SearchWarp's field reads stay on-chip; the scan's per_warp_smem layout follows in the dynamic window,
+ * which the host sizes to the largest per_warp_smem of the launch.  The kernel clears the scan's overflow word, which
+ * dann_scan_gettuple clears with a memset before its launch.  Register budget: 168 per thread, the one
+ * dann_search_kernel's (384, 1) bound gives the same code (with a bare 32-thread bound ptxas settles on 128 for some
+ * Ent64 instantiations and spills). */
+template <typename T, int NCH, int PLAIN = 0>
+__global__ void __launch_bounds__(32, 12) dann_scan_search_many_kernel(const SearchArgs *args, uint32_t nscans) {
+    DANN_DYN_SMEM(dann_smem);
+    DANN_STATIC_SMEM __align__(16) unsigned char s_args[sizeof(SearchArgs)];
+    static_assert(sizeof(SearchArgs) % 8 == 0, "SearchArgs is copied in 8-byte words");
+    if (blockIdx.x >= nscans) return;
+    const int lane = threadIdx.x & 31;
+    const uint64_t *src = reinterpret_cast<const uint64_t *>(args + blockIdx.x);
+    uint64_t *dst = reinterpret_cast<uint64_t *>(s_args);
+    for (uint32_t i = lane; i < sizeof(SearchArgs) / 8; i += 32) dst[i] = src[i];
+    __syncwarp();
+    const SearchArgs &a = *reinterpret_cast<const SearchArgs *>(s_args);
+    if (lane == 0) *a.overflow = 0u;
+    __syncwarp();
+    SearchWarp<T, NCH, PLAIN> w(a, lane);
+    bind_search_warp(w, a, dann_smem, 0u);
+    w.run(0u);
 }

@@ -12,6 +12,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <functional>
 #include <mutex>
 #include <new>
 #include <string>
@@ -176,6 +177,8 @@ struct dann_index {
     bool plain = false;
     const float *index_vectors = nullptr; /* [n][dim_index] in HBM */
     DevBuf sc_qindex;
+    /* dann_scan_gettuple_many: one round's per-scan launch arguments and descriptors, then its ScanStepOut array */
+    DevBuf sc_many;
 };
 
 
@@ -271,7 +274,7 @@ extern "C" void dann_index_free(dann_index *ix) {
     DevBuf *bufs[] = {&ix->ws_hash, &ix->ws_cand, &ix->ws_heap, &ix->ws_bitmap, &ix->ws_ins, &ix->sc_qfull, &ix->sc_qcodes,
                       &ix->sc_stream, &ix->sc_stream_len, &ix->sc_stats, &ix->sc_qlist, &ix->sc_ctl,
                       &ix->sc_node, &ix->sc_qindex, &ix->st_queries, &ix->st_labels, &ix->st_label_off, &ix->st_tid,
-                      &ix->st_dist, &ix->st_count, &ix->st_stats};
+                      &ix->st_dist, &ix->st_count, &ix->st_stats, &ix->sc_many};
     for (DevBuf *b : bufs) b->release();
     for (auto &e : ix->ev)
         if (e) cudaEventDestroy(e);
@@ -625,6 +628,23 @@ static search_fn pick_kernel(bool pairs, int entry, uint32_t nch, bool plain = f
     if (plain) return dann_search_kernel<Ent64, 1, 1>;
     if (pairs) return entry == 0 ? pick_search2<Ent32x21>(nch) : entry == 1 ? pick_search2<Ent32x16>(nch) : pick_search2<Ent64>(nch);
     return entry == 0 ? pick_search<Ent32x21>(nch) : entry == 1 ? pick_search<Ent32x16>(nch) : pick_search<Ent64>(nch);
+}
+
+/* dann_scan_search_many_kernel: the instantiations pick_kernel(false, ...) offers the streaming scan */
+typedef void (*scan_many_fn)(const SearchArgs *, uint32_t);
+template <typename T>
+static scan_many_fn pick_scan_many_t(uint32_t nch) {
+    switch (nch) {
+        case 1: return dann_scan_search_many_kernel<T, 1>;
+        case 2: return dann_scan_search_many_kernel<T, 2>;
+        case 3: return dann_scan_search_many_kernel<T, 3>;
+        case 4: return dann_scan_search_many_kernel<T, 4>;
+        default: return dann_scan_search_many_kernel<T, 8>;
+    }
+}
+static scan_many_fn pick_scan_many(int entry, uint32_t nch, bool plain) {
+    if (plain) return dann_scan_search_many_kernel<Ent64, 1, 1>;
+    return entry == 0 ? pick_scan_many_t<Ent32x21>(nch) : entry == 1 ? pick_scan_many_t<Ent32x16>(nch) : pick_scan_many_t<Ent64>(nch);
 }
 
 template <typename T, int MAXW>
@@ -1295,16 +1315,15 @@ extern "C" int dann_scan_rescan(dann_scan *sc, const float *query, const int16_t
     return DANN_OK;
 } DANN_CATCH
 
-/* Enqueue the resumable search for rows [0, want) of this launch (d_ctl[1] receives the overflow bits). */
-static int scan_launch_search(dann_scan *sc, uint32_t want) {
+/* The launch arguments of the scan's resumable search for rows [0, want) of this step: its plan, its private workspace
+ * and its saved state (d_ctl[1] receives the overflow bits). */
+static int scan_search_args(dann_scan *sc, uint32_t want, SearchArgs *out) {
     dann_index *ix = sc->ix;
     const IndexView &v = ix->v;
-    cudaStream_t st = ix->stream;
     {
         const SearchPlan &p = sc->plan;
         CK(sc->d_stream.reserve((size_t)want * 4));
         uint32_t *d_ctl = sc->d_ctl.as<uint32_t>();
-        CK(cudaMemsetAsync(d_ctl, 0, 8, st));
         SearchArgs a = search_args_for_plan(v, ix->G, ix->Gshift, ix->lists_unique, p);
         a.q_codes = sc->d_qcodes.as<uint64_t>();
         a.q_labels = sc->nlabels >= 0 ? sc->d_labels.as<int16_t>() : nullptr;
@@ -1328,13 +1347,94 @@ static int scan_launch_search(dann_scan *sc, uint32_t want) {
         a.plain_vectors = ix->index_vectors;
         a.q_index = sc->d_qindex.as<float>();
         a.plain_dim = ix->plain ? v.dim_index : 0;
-        search_fn fn = pick_kernel(false, p.entry, ix->NCH, ix->plain);
-        CK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(p.per_warp + DANN_SMEM_SLACK)));
-        fn<<<1, 32, p.per_warp + DANN_SMEM_SLACK, st>>>(a);
-        ix->launches++;
-        CK(cudaGetLastError());
+        *out = a;
     }
     return DANN_OK;
+}
+
+/* Enqueue the resumable search for rows [0, want) of this launch (d_ctl[1] receives the overflow bits). */
+static int scan_launch_search(dann_scan *sc, uint32_t want) {
+    dann_index *ix = sc->ix;
+    cudaStream_t st = ix->stream;
+    const SearchPlan &p = sc->plan;
+    SearchArgs a;
+    int rc = scan_search_args(sc, want, &a);
+    if (rc) return rc;
+    CK(cudaMemsetAsync(sc->d_ctl.p, 0, 8, st));
+    search_fn fn = pick_kernel(false, p.entry, ix->NCH, ix->plain);
+    CK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(p.per_warp + DANN_SMEM_SLACK)));
+    fn<<<1, 32, p.per_warp + DANN_SMEM_SLACK, st>>>(a);
+    ix->launches++;
+    CK(cudaGetLastError());
+    return DANN_OK;
+}
+
+/* rows this amgettuple takes off the approximate stream: next_with_resort refills the window to `rescore`
+ * (scan.rs:255-305), next() takes one */
+static uint32_t scan_step_need(const dann_scan *sc) {
+    const uint32_t rescore = (uint32_t)sc->rescore;
+    return rescore == 0 ? 1u : (sc->win_len < rescore ? rescore - sc->win_len : 0u);
+}
+
+/* dynamic shared memory of a scan-distance CTA: the query row */
+static size_t scan_distance_smem(const IndexView &v) { return (size_t)((v.dim + 3u) & ~3u) * sizeof(float) + DANN_SMEM_SLACK; }
+
+/* the arguments of the exact distances of the rows [skip, want) a search step may append */
+static int scan_distance_desc(dann_scan *sc, uint32_t want, uint32_t skip, ScanDistanceDesc *d) {
+    dann_index *ix = sc->ix;
+    CK(sc->d_dist.reserve((size_t)want * 4));
+    *d = ScanDistanceDesc{sc->d_qfull.as<float>(), sc->d_stream.as<uint32_t>(), sc->d_slen.as<uint32_t>(),
+                          sc->d_ctl.as<uint32_t>() + 1, sc->d_dist.as<float>(), skip, 0u};
+    return DANN_OK;
+}
+
+/* the arguments of the window step; a step that does not search finds nothing new beyond `skip` */
+static ScanFinishDesc scan_finish_desc(dann_scan *sc, bool searching, uint32_t skip) {
+    ScanFinishDesc f;
+    f.w = sc->d_winst.as<ScanWindow>();
+    f.win = sc->d_win.as<uint64_t>();
+    f.stream = sc->d_stream.as<uint32_t>();
+    f.dist = sc->d_dist.as<float>();
+    f.slen_p = searching ? sc->d_slen.as<uint32_t>() : nullptr;
+    f.overflow_p = searching ? sc->d_ctl.as<uint32_t>() + 1 : nullptr;
+    f.stats_p = sc->d_stats.as<dann_query_stats>();
+    f.rescore = (uint32_t)sc->rescore;
+    f.skip = skip;
+    f.slen_fixed = skip;
+    f.pad = 0;
+    return f;
+}
+
+/* the scan outgrew its workspace: rebuild it twice as large; the next search replays the stream up to sc->streamed */
+static int scan_regrow(dann_scan *sc, int attempt) {
+    if (attempt >= 8) return fail(DANN_ERR_CAPACITY, "scan workspace still too small after %d growth steps", attempt);
+    sc->grow *= 2;
+    return scan_reset_search(sc);
+}
+
+/* The host side of a step that did not overflow: the stream position, end of stream and counters of the scan, then its
+ * row.  `want` = rows [0, want) the search was asked for, the first `skip` of them replayed.  Returns 1 (row) or 0
+ * (end of scan). */
+static int scan_after_step(dann_scan *sc, const ScanStepOut &o, bool searching, uint32_t want, uint32_t skip,
+                           uint32_t *block, uint16_t *offset, uint32_t *node_id, float *dist) {
+    if (searching) {
+        if (o.slen < want) sc->exhausted = true;
+        sc->streamed += o.slen > skip ? o.slen - skip : 0;
+        sc->stats = o.stats;
+    }
+    sc->win_len = o.win.len;
+    sc->stats.d_full = o.win.d_full;
+    if (sc->ix->plain) { /* every comparison of the beam search was a full-distance comparison (plain/storage.rs:238,288) */
+        sc->stats.d_full += sc->stats.candidates;
+        sc->stats.d_quantized = 0;
+    }
+    sc->stats.stream_len = sc->streamed;
+    if (!o.row.have) return 0;
+    if (block) *block = (uint32_t)(o.row.tid >> 16);
+    if (offset) *offset = (uint16_t)(o.row.tid & 0xFFFFu);
+    if (node_id) *node_id = o.row.node;
+    if (dist) *dist = o.row.dist;
+    return 1;
 }
 
 /* next_with_resort (scan.rs:244-305): `while resort_buffer.len() < resort_size { next() ... }` then pop; with
@@ -1349,8 +1449,7 @@ extern "C" int dann_scan_gettuple(dann_scan *sc, uint32_t *block, uint16_t *offs
     std::lock_guard<std::mutex> lk(ix->mu);
     const IndexView &v = ix->v;
     cudaStream_t st = ix->stream;
-    const uint32_t rescore = (uint32_t)sc->rescore;
-    const uint32_t need = rescore == 0 ? 1u : (sc->win_len < rescore ? rescore - sc->win_len : 0u);
+    const uint32_t need = scan_step_need(sc);
     const bool searching = need && !sc->exhausted;
     ScanStepOut o;
     uint32_t skip = 0; /* rows that are only re-generated because the workspace had to grow */
@@ -1359,54 +1458,222 @@ extern "C" int dann_scan_gettuple(dann_scan *sc, uint32_t *block, uint16_t *offs
         if (searching) {
             rc = scan_launch_search(sc, want);
             if (rc) return rc;
-            if (rescore > 0) {
-                CK(sc->d_dist.reserve((size_t)want * 4));
-                size_t smem = (size_t)((v.dim + 3u) & ~3u) * sizeof(float) + DANN_SMEM_SLACK;
+            if (sc->rescore > 0) {
+                ScanDistanceDesc d;
+                rc = scan_distance_desc(sc, want, skip, &d);
+                if (rc) return rc;
+                const size_t smem = scan_distance_smem(v);
                 CK(allow_dynamic_smem(dann_scan_distance_kernel, smem));
-                dann_scan_distance_kernel<<<1, 128, smem, st>>>(v, sc->d_qfull.as<float>(), sc->d_stream.as<uint32_t>(),
-                                                               sc->d_slen.as<uint32_t>(), sc->d_ctl.as<uint32_t>() + 1, skip,
-                                                               sc->d_dist.as<float>());
+                dann_scan_distance_kernel<<<1, 128, smem, st>>>(v, d.q_full, d.stream, d.slen_p, d.overflow_p, d.skip, d.out);
                 ix->launches++;
                 CK(cudaGetLastError());
             }
         }
-        dann_scan_finish_kernel<<<1, 32, 0, st>>>(v, sc->d_winst.as<ScanWindow>(), sc->d_win.as<uint64_t>(), rescore,
-                                                 sc->d_stream.as<uint32_t>(), sc->d_dist.as<float>(), skip,
-                                                 searching ? sc->d_slen.as<uint32_t>() : nullptr, skip,
-                                                 searching ? sc->d_ctl.as<uint32_t>() + 1 : nullptr,
-                                                 sc->d_stats.as<dann_query_stats>(), sc->d_step.as<ScanStepOut>());
+        const ScanFinishDesc f = scan_finish_desc(sc, searching, skip);
+        dann_scan_finish_kernel<<<1, 32, 0, st>>>(v, f.w, f.win, f.rescore, f.stream, f.dist, f.skip, f.slen_p, f.slen_fixed,
+                                                 f.overflow_p, f.stats_p, sc->d_step.as<ScanStepOut>());
         ix->launches++;
         CK(cudaGetLastError());
         CK(cudaMemcpyAsync(&o, sc->d_step.p, sizeof o, cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
-        if (!o.overflow) {
-            if (searching) {
-                if (o.slen < want) sc->exhausted = true;
-                sc->streamed += o.slen > skip ? o.slen - skip : 0;
-                sc->stats = o.stats;
-            }
-            break;
-        }
-        /* the scan outgrew its workspace: rebuild it twice as large and replay the stream up to here */
-        if (attempt >= 8) return fail(DANN_ERR_CAPACITY, "scan workspace still too small after %d growth steps", attempt);
-        sc->grow *= 2;
-        rc = scan_reset_search(sc);
+        if (!o.overflow) break;
+        rc = scan_regrow(sc, attempt);
         if (rc) return rc;
         skip = sc->streamed;
     }
-    sc->win_len = o.win.len;
-    sc->stats.d_full = o.win.d_full;
-    if (ix->plain) { /* every comparison of the beam search was a full-distance comparison (plain/storage.rs:238,288) */
-        sc->stats.d_full += sc->stats.candidates;
-        sc->stats.d_quantized = 0;
+    return scan_after_step(sc, o, searching, skip + need, skip, block, offset, node_id, dist);
+} DANN_CATCH
+
+/* The device part of one dann_scan_gettuple_many round: one upload of [SearchArgs x args][ScanDistanceDesc x ddesc]
+ * [ScanFinishDesc x fdesc], one dann_scan_search_many_kernel launch per run of equal fns[] (args is grouped by
+ * instantiation), one dann_scan_distance_many_kernel launch when ddesc is not empty, one dann_scan_finish_many_kernel
+ * launch, one download of the fdesc.size() outcomes into outs and one synchronisation. */
+static int scan_many_round(dann_index *ix, const std::vector<scan_many_fn> &fns, const std::vector<SearchArgs> &args,
+                           const std::vector<ScanDistanceDesc> &ddesc, const std::vector<ScanFinishDesc> &fdesc,
+                           std::vector<unsigned char> &blob, std::vector<ScanStepOut> &outs) {
+    const IndexView &v = ix->v;
+    cudaStream_t st = ix->stream;
+    const size_t m = fdesc.size();
+    auto align16 = [](size_t b) { return (b + 15) & ~(size_t)15; };
+    const size_t o_dist = align16(args.size() * sizeof(SearchArgs));
+    const size_t o_fin = o_dist + align16(ddesc.size() * sizeof(ScanDistanceDesc));
+    const size_t o_out = o_fin + align16(m * sizeof(ScanFinishDesc));
+    blob.assign(o_out, 0);
+    if (!args.empty()) memcpy(blob.data(), args.data(), args.size() * sizeof(SearchArgs));
+    if (!ddesc.empty()) memcpy(blob.data() + o_dist, ddesc.data(), ddesc.size() * sizeof(ScanDistanceDesc));
+    memcpy(blob.data() + o_fin, fdesc.data(), m * sizeof(ScanFinishDesc));
+    CK(ix->sc_many.reserve(o_out + m * sizeof(ScanStepOut)));
+    unsigned char *dev = ix->sc_many.as<unsigned char>();
+    CK(cudaMemcpyAsync(dev, blob.data(), o_out, cudaMemcpyHostToDevice, st));
+    for (size_t g = 0; g < args.size();) {
+        size_t e = g;
+        uint32_t per_warp = 0;
+        for (; e < args.size() && fns[e] == fns[g]; e++) per_warp = std::max(per_warp, args[e].per_warp_smem);
+        const scan_many_fn fn = fns[g];
+        const size_t smem = (size_t)per_warp + DANN_SMEM_SLACK;
+        CK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        fn<<<(unsigned)(e - g), 32, smem, st>>>(reinterpret_cast<const SearchArgs *>(dev) + g, (uint32_t)(e - g));
+        ix->launches++;
+        CK(cudaGetLastError());
+        g = e;
     }
-    sc->stats.stream_len = sc->streamed;
-    if (!o.row.have) return 0;
-    if (block) *block = (uint32_t)(o.row.tid >> 16);
-    if (offset) *offset = (uint16_t)(o.row.tid & 0xFFFFu);
-    if (node_id) *node_id = o.row.node;
-    if (dist) *dist = o.row.dist;
-    return 1;
+    if (!ddesc.empty()) {
+        const size_t smem = scan_distance_smem(v);
+        CK(allow_dynamic_smem(dann_scan_distance_many_kernel, smem));
+        dann_scan_distance_many_kernel<<<(unsigned)ddesc.size(), 128, smem, st>>>(
+            v, reinterpret_cast<const ScanDistanceDesc *>(dev + o_dist));
+        ix->launches++;
+        CK(cudaGetLastError());
+    }
+    dann_scan_finish_many_kernel<<<(unsigned)((m + 127) / 128), 128, 0, st>>>(
+        v, reinterpret_cast<const ScanFinishDesc *>(dev + o_fin), (uint32_t)m, reinterpret_cast<ScanStepOut *>(dev + o_out));
+    ix->launches++;
+    CK(cudaGetLastError());
+    outs.resize(m);
+    CK(cudaMemcpyAsync(outs.data(), dev + o_out, m * sizeof(ScanStepOut), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    return DANN_OK;
+}
+
+/* One amgettuple of each of n scans of one index, in rounds (scan_many_round).  The first round takes every scan; a
+ * scan whose search overflowed regrows alone and replays in the next round, with the others done.
+ * What fails for one scan (its workspace cannot grow, or its buffers cannot be allocated) goes to that scan's out_rc
+ * and, when msgs != NULL, its message to (*msgs)[i]; the other scans go on.  A failure of a round as a whole fails the
+ * call only while no scan has taken its step yet; after that it goes to the out_rc of every scan of the round, so that
+ * no scan's row is lost. */
+static int scan_gettuple_many(dann_scan *const *scans, int n, int32_t *out_rc, uint32_t *block, uint16_t *offset,
+                              uint32_t *node_id, float *dist, std::vector<std::string> *msgs) {
+    if (!scans || !out_rc) return fail(DANN_ERR_INVALID_ARG, "dann_scan_gettuple_many: NULL argument");
+    if (n < 1 || n > 65536) return fail(DANN_ERR_INVALID_ARG, "dann_scan_gettuple_many: n = %d outside 1..65536", n);
+    for (int i = 0; i < n; i++)
+        if (!scans[i]) return fail(DANN_ERR_INVALID_ARG, "dann_scan_gettuple_many: scan %d is NULL", i);
+    dann_index *ix = scans[0]->ix;
+    for (int i = 1; i < n; i++)
+        if (scans[i]->ix != ix) return fail(DANN_ERR_INVALID_ARG, "dann_scan_gettuple_many: scans 0 and %d belong to different indexes", i);
+    {
+        std::vector<dann_scan *> sorted(scans, scans + n);
+        std::sort(sorted.begin(), sorted.end(), std::less<dann_scan *>());
+        if (std::adjacent_find(sorted.begin(), sorted.end()) != sorted.end())
+            return fail(DANN_ERR_INVALID_ARG, "dann_scan_gettuple_many: a scan appears twice");
+    }
+    for (int i = 0; i < n; i++)
+        if (!scans[i]->active) return fail(DANN_ERR_STATE, "dann_scan_gettuple_many: scan %d has not been rescanned", i);
+    int rc = check_live(ix);
+    if (rc) return rc;
+    std::lock_guard<std::mutex> lk(ix->mu);
+
+    struct Step {
+        dann_scan *sc;
+        int i;            /* position in the caller's arrays */
+        uint32_t need, skip;
+        bool searching;
+        int attempt;
+        scan_many_fn fn;  /* its search instantiation */
+    };
+    /* everything the rounds use is allocated here, before any scan moves: a host allocation failure later would fail
+     * the call after some scans have taken their step */
+    std::vector<Step> steps((size_t)n);
+    std::vector<Step *> round((size_t)n), searchers, live, next;
+    std::vector<scan_many_fn> fns;
+    std::vector<SearchArgs> args;
+    std::vector<ScanDistanceDesc> ddesc;
+    std::vector<ScanFinishDesc> fdesc;
+    std::vector<unsigned char> blob;
+    std::vector<ScanStepOut> outs;
+    searchers.reserve(n);
+    live.reserve(n);
+    next.reserve(n);
+    fns.reserve(n);
+    args.reserve(n);
+    ddesc.reserve(n);
+    fdesc.reserve(n);
+    outs.reserve(n);
+    blob.reserve((size_t)n * (sizeof(SearchArgs) + sizeof(ScanDistanceDesc) + sizeof(ScanFinishDesc)) + 64);
+    if (msgs) msgs->assign((size_t)n, std::string());
+    for (int i = 0; i < n; i++) {
+        dann_scan *sc = scans[i];
+        const uint32_t need = scan_step_need(sc);
+        steps[i] = Step{sc, i, need, 0u, need && !sc->exhausted, 0, nullptr};
+        round[i] = &steps[i];
+    }
+    bool moved = false; /* some scan has taken its step */
+    auto scan_failed = [&](const Step *s, int code) {
+        out_rc[s->i] = code;
+        if (msgs) {
+            try {
+                (*msgs)[s->i] = g_err;
+            } catch (...) { /* no memory for the message: the code still goes back */
+            }
+        }
+    };
+    while (!round.empty()) {
+        /* the searching scans, grouped by instantiation: one launch per group */
+        searchers.clear();
+        for (Step *s : round)
+            if (s->searching) {
+                s->fn = pick_scan_many(s->sc->plan.entry, ix->NCH, ix->plain);
+                searchers.push_back(s);
+            }
+        std::stable_sort(searchers.begin(), searchers.end(),
+                         [](const Step *a, const Step *b) { return (uintptr_t)a->fn < (uintptr_t)b->fn; });
+        fns.clear();
+        args.clear();
+        ddesc.clear();
+        for (Step *s : searchers) {
+            const uint32_t want = s->skip + s->need;
+            SearchArgs a;
+            ScanDistanceDesc d{};
+            rc = scan_search_args(s->sc, want, &a);
+            if (!rc && s->sc->rescore > 0) rc = scan_distance_desc(s->sc, want, s->skip, &d);
+            if (rc) { /* this scan's buffers: it leaves the round */
+                scan_failed(s, rc);
+                s->fn = nullptr;
+                continue;
+            }
+            fns.push_back(s->fn);
+            args.push_back(a);
+            if (s->sc->rescore > 0) ddesc.push_back(d);
+        }
+        live.clear();
+        fdesc.clear();
+        for (Step *s : round)
+            if (!s->searching || s->fn) {
+                live.push_back(s);
+                fdesc.push_back(scan_finish_desc(s->sc, s->searching, s->skip));
+            }
+        if (live.empty()) break;
+        rc = scan_many_round(ix, fns, args, ddesc, fdesc, blob, outs);
+        if (rc) {
+            if (!moved) return rc;
+            for (Step *s : live) scan_failed(s, rc);
+            break;
+        }
+        next.clear();
+        for (size_t j = 0; j < live.size(); j++) {
+            Step *s = live[j];
+            const int i = s->i;
+            if (!outs[j].overflow) {
+                out_rc[i] = scan_after_step(s->sc, outs[j], s->searching, s->skip + s->need, s->skip, block ? block + i : nullptr,
+                                            offset ? offset + i : nullptr, node_id ? node_id + i : nullptr, dist ? dist + i : nullptr);
+                moved = true;
+                continue;
+            }
+            rc = scan_regrow(s->sc, s->attempt++);
+            if (rc) { /* capacity, memory, or a CUDA error that has poisoned the handle: this scan alone */
+                scan_failed(s, rc);
+                continue;
+            }
+            s->skip = s->sc->streamed;
+            next.push_back(s);
+        }
+        round.swap(next);
+    }
+    return DANN_OK;
+}
+
+extern "C" int dann_scan_gettuple_many(dann_scan *const *scans, int n, int32_t *out_rc, uint32_t *block, uint16_t *offset,
+                                       uint32_t *node_id, float *dist) try {
+    return scan_gettuple_many(scans, n, out_rc, block, offset, node_id, dist, nullptr);
 } DANN_CATCH
 
 extern "C" int dann_scan_stats(dann_scan *sc, dann_query_stats *out) try {

@@ -72,8 +72,8 @@ STATS_DTYPE = np.dtype([("visits", "<u4"), ("d_quantized", "<u4"), ("candidates"
 EXPORTS = [
     "dann_last_error", "dann_device_count", "dann_index_load", "dann_index_load_plain", "dann_index_free",
     "dann_coalescer_create", "dann_coalescer_search", "dann_coalescer_stats", "dann_coalescer_destroy",
-    "dann_index_hbm_bytes", "dann_scan_begin", "dann_scan_rescan", "dann_scan_gettuple",
-    "dann_scan_stats", "dann_scan_end", "dann_search_batch", "dann_search_batch_device",
+    "dann_index_hbm_bytes", "dann_scan_begin", "dann_scan_rescan", "dann_scan_gettuple", "dann_scan_gettuple_many",
+    "dann_coalescer_gettuple", "dann_scan_stats", "dann_scan_end", "dann_search_batch", "dann_search_batch_device",
     "dann_prepare_queries", "dann_code_stride", "dann_sbq_distance", "dann_full_distance",
     "dann_kernel_launches", "dann_last_batch_timing",
     "dann_build_graph", "dann_index_download_nbrs", "dann_index_set_vectors", "dann_index_set_vectors_device",
@@ -113,6 +113,7 @@ def load_library(path: Optional[str] = None):
     lib.dann_scan_begin.argtypes = [vp, C.POINTER(vp)]
     lib.dann_scan_rescan.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int]
     lib.dann_scan_gettuple.argtypes = [vp, u32p, C.POINTER(C.c_uint16), u32p, C.POINTER(C.c_float)]
+    lib.dann_scan_gettuple_many.argtypes = [vp, C.c_int, vp, vp, vp, vp, vp]
     lib.dann_scan_stats.argtypes = [vp, C.POINTER(_QueryStats)]
     lib.dann_scan_end.argtypes = [vp]
     lib.dann_scan_end.restype = None
@@ -137,6 +138,7 @@ def load_library(path: Optional[str] = None):
     lib.dann_group_free.restype = None
     lib.dann_coalescer_create.argtypes = [vp, C.c_int, C.c_int, C.POINTER(vp)]
     lib.dann_coalescer_search.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp]
+    lib.dann_coalescer_gettuple.argtypes = [vp, vp, u32p, C.POINTER(C.c_uint16), u32p, C.POINTER(C.c_float)]
     lib.dann_coalescer_stats.argtypes = [vp, vp, vp, vp]
     lib.dann_coalescer_destroy.argtypes = [vp]
     lib.dann_coalescer_destroy.restype = None
@@ -421,6 +423,34 @@ class IndexScan:
             pass
 
 
+def gettuple_many(scans: Sequence["IndexScan"]) -> list:
+    """One amgettuple of each scan (all of one index) in one call (dann_scan_gettuple_many): the suspended searches
+    resume together on the GPU.  Returns one entry per scan: the row as IndexScan.gettuple gives it, None at end of
+    scan, or that scan's DiskAnnError (returned, not raised; its code is the scan's own, its message the call's last
+    failure, dann_last_error).  Errors of the call itself raise."""
+    scans = list(scans)
+    n = len(scans)
+    lib = scans[0]._lib if n else load_library()
+    handles = (C.c_void_p * max(n, 1))(*[s._h for s in scans])
+    rc = np.zeros(max(n, 1), np.int32)
+    block = np.zeros(max(n, 1), np.uint32)
+    offset = np.zeros(max(n, 1), np.uint16)
+    node = np.zeros(max(n, 1), np.uint32)
+    dist = np.zeros(max(n, 1), np.float32)
+    _check(lib, lib.dann_scan_gettuple_many(handles, n, _np_ptr(rc), _np_ptr(block), _np_ptr(offset), _np_ptr(node),
+                                            _np_ptr(dist)))
+    err = lib.dann_last_error().decode("utf-8", "replace")
+    out = []
+    for i in range(n):
+        if rc[i] < 0:
+            out.append(DiskAnnError(int(rc[i]), err))
+        elif rc[i] == 0:
+            out.append(None)
+        else:
+            out.append((int(block[i]), int(offset[i]), int(node[i]), float(dist[i])))
+    return out
+
+
 class IndexGroup:
     """dann_group: one replica of the index per GPU inside this process; a batch is split into contiguous slices, every
     device runs the whole hot path on its slice, rows come back in query order (SURVEY.md §8b / §8e)."""
@@ -496,7 +526,18 @@ class Coalescer:
         return dict(tid=tid, dist=dist, count=int(count.value),
                     stats={f: int(getattr(st, f)) for f, _ in _QueryStats._fields_})
 
+    def gettuple(self, scan: "IndexScan"):
+        """IndexScan.gettuple through the dispatcher: gettuple calls of many threads (any scans of this index) that
+        arrive together become one dann_scan_gettuple_many.  Blocks; returns what scan.gettuple() would."""
+        b, o, n, d = C.c_uint32(), C.c_uint16(), C.c_uint32(), C.c_float()
+        rc = _check(self._lib, self._lib.dann_coalescer_gettuple(self._h, scan._h, C.byref(b), C.byref(o), C.byref(n),
+                                                                 C.byref(d)))
+        if rc == 0:
+            return None
+        return int(b.value), int(o.value), int(n.value), float(d.value)
+
     def stats(self) -> dict:
+        """batches / queries / largest_batch count search and gettuple dispatches alike."""
         b, q, m = C.c_uint64(), C.c_uint64(), C.c_uint64()
         _check(self._lib, self._lib.dann_coalescer_stats(self._h, C.byref(b), C.byref(q), C.byref(m)))
         return dict(batches=int(b.value), queries=int(q.value), largest_batch=int(m.value))
