@@ -749,6 +749,8 @@ struct Builder {
     bool have_start = false;
     uint32_t start_default = ORC_INVALID_NODE;
     std::map<int16_t, uint32_t> start_labeled; /* BTreeMap */
+    orc_build_switches sw{};   /* all zero: the reference's rules (orc_build never sets one) */
+    uint64_t bc[ORC_BC_N] = {}; /* branch counters, see oracle.h */
 
     const int16_t *labs(uint32_t i, uint32_t *cnt) const {
         if (!has_labels) {
@@ -763,12 +765,21 @@ struct Builder {
         return (float)orc_hamming(codes + (size_t)a * words, codes + (size_t)b * words, words);
     }
 
+    void sort_candidates(std::vector<Nwd> &cand) const {
+        if (sw.order_by_id)
+            std::sort(cand.begin(), cand.end(), [](const Nwd &a, const Nwd &b) {
+                return a.d.d != b.d.d ? a.d.d < b.d.d : a.node < b.node;
+            });
+        else
+            std::stable_sort(cand.begin(), cand.end(),
+                             [](const Nwd &a, const Nwd &b) { return dwtb_cmp(a.d, b.d) < 0; });
+    }
+
     /* graph/mod.rs:392-488 */
     std::vector<Nwd> prune(uint32_t point, std::vector<Nwd> cand) {
         uint32_t np;
         const int16_t *pl = labs(point, &np);
-        std::stable_sort(cand.begin(), cand.end(),
-                         [](const Nwd &a, const Nwd &b) { return dwtb_cmp(a.d, b.d) < 0; });
+        sort_candidates(cand);
         std::vector<Nwd> results;
         results.reserve(R);
         std::vector<double> max_factors(cand.size(), 0.0);
@@ -779,6 +790,7 @@ struct Builder {
                 if (max_factors[i] > alpha) continue;
                 max_factors[i] = 1.7976931348623157e308;
                 results.push_back(cand[i]);
+                if (alpha > 1.0) bc[ORC_BC_ROUND2_KEPT]++;
                 const Nwd &ex = cand[i];
                 uint32_t ne;
                 const int16_t *el = labs(ex.node, &ne);
@@ -787,9 +799,13 @@ struct Builder {
                     if (has_labels) {
                         uint32_t nc;
                         const int16_t *cl = labs(cand[j].node, &nc);
-                        if (!orc_labels_contains_intersection(el, ne, cl, nc, pl, np)) continue;
+                        if (!orc_labels_contains_intersection(el, ne, cl, nc, pl, np)) {
+                            bc[ORC_BC_LABEL_SKIP]++;
+                            continue;
+                        }
                     }
                     float raw = ham(ex.node, cand[j].node);
+                    if (raw == 0.0f) bc[cand[j].d.d == 0.0f ? ORC_BC_TIE_FACTOR : ORC_BC_ZERO_OCCLUDED]++;
                     Dwtb between{raw, ipd(cand[j].node, ex.node)};
                     double factor = dwtb_factor(cand[j].d, between);
                     max_factors[j] = std::max(max_factors[j], factor);
@@ -800,8 +816,14 @@ struct Builder {
         return results;
     }
 
-    /* graph/mod.rs:212-266 */
     std::vector<Nwd> add_neighbors(uint32_t of, const std::vector<Nwd> &additional) {
+        return add_neighbors(of, additional, max_during_build, false, nullptr);
+    }
+
+    /* graph/mod.rs:212-266.  `keep` = the length above which the list is pruned (the reference:
+     * max_neighbors_during_build); `store_sorted` = the merged list is put in candidate order first */
+    std::vector<Nwd> add_neighbors(uint32_t of, const std::vector<Nwd> &additional, size_t keep, bool store_sorted,
+                                   bool *pruned) {
         std::vector<Nwd> cand = nbrs[of];
         std::unordered_set<uint32_t> hash;
         for (auto &c : cand) hash.insert(c.node);
@@ -814,7 +836,9 @@ struct Builder {
                     break;
                 }
         }
-        std::vector<Nwd> out = cand.size() > max_during_build ? prune(of, cand) : cand;
+        if (store_sorted) sort_candidates(cand);
+        if (pruned) *pruned = cand.size() > keep;
+        std::vector<Nwd> out = cand.size() > keep ? prune(of, cand) : cand;
         nbrs[of] = out;
         return out;
     }
@@ -840,7 +864,7 @@ struct Builder {
             if (!l.prepare_insert(sn)) continue;
             l.stats.d_quantized++;
             float d = (float)orc_hamming(codes + (size_t)sn * words, qc, words);
-            l.insert_neighbor(Lsn{sn, Dwtb{d, ipd(sn, ip)}});
+            l.insert_neighbor(Lsn{sn, Dwtb{d, sw.scan_ties ? 0 : ipd(sn, ip)}});
         }
         long idx;
         while ((idx = l.visit_closest(L)) >= 0) {
@@ -856,9 +880,20 @@ struct Builder {
                 }
                 l.stats.d_quantized++;
                 float d = (float)orc_hamming(codes + (size_t)nb.node * words, qc, words);
-                l.insert_neighbor(Lsn{nb.node, Dwtb{d, ipd(nb.node, ip)}});
+                l.insert_neighbor(Lsn{nb.node, Dwtb{d, sw.scan_ties ? 0 : ipd(nb.node, ip)}});
             }
         }
+        if (sw.visited_cap || sw.cand_cap) { /* the distance-ordered visited list itself, possibly cut short */
+            size_t nv = l.visited.size();
+            if (sw.visited_cap && nv > sw.visited_cap) {
+                nv = sw.visited_cap;
+                bc[ORC_BC_VISITED_CUT]++;
+            }
+            visited_nodes.clear();
+            for (size_t i = 0; i < nv; i++) visited_nodes.push_back(Nwd{l.visited[i].node, l.visited[i].d});
+        }
+        for (Nwd &v : visited_nodes) v.d.tie = ipd(v.node, ip); /* the prune's tie-break, whatever ordered the search */
+        if (visited_nodes.empty()) bc[ORC_BC_EMPTY_SEARCH]++;
         /* HashSet<NeighborWithDistance> keyed by pointer: dedupe (cannot repeat here) */
         return visited_nodes;
     }
@@ -884,6 +919,62 @@ struct Builder {
                 if (!start_labeled.count(l[i])) start_labeled[l[i]] = ip;
         if (has_labels) insert_internal(ip, false);
         insert_internal(ip, true);
+    }
+
+    /* insert_internal for the nodes [lo, lo + m) at once: all searches first (none sees a batch mate's edges),
+     * then the forward lists, then the back-links per destination in (distance, source) order */
+    void insert_batch(uint32_t lo, uint32_t m, bool no_filter) {
+        const size_t cap13 = max_during_build;
+        const size_t back_keep = sw.slots ? std::min<size_t>(sw.slots, cap13) : cap13;
+        const size_t fwd_keep = sw.fwd_keep_slots ? sw.slots : back_keep;
+        std::vector<std::vector<Nwd>> vis(m);
+        for (uint32_t b = 0; b < m; b++) vis[b] = search_for_build(lo + b, no_filter);
+        struct Trip {
+            uint32_t dst;
+            float d;
+            uint32_t src;
+        };
+        std::vector<Trip> trips;
+        for (uint32_t b = 0; b < m; b++) {
+            const uint32_t p = lo + b;
+            std::vector<Nwd> &v = vis[b];
+            const size_t deg = nbrs[p].size();
+            if (deg) bc[ORC_BC_FWD_MERGED]++;
+            if (sw.cand_cap && v.size() > sw.cand_cap - deg) {
+                v.resize(sw.cand_cap - deg);
+                bc[ORC_BC_CAND_CUT]++;
+            }
+            bool pruned;
+            std::vector<Nwd> list = add_neighbors(p, v, fwd_keep, sw.order_by_id != 0, &pruned);
+            bc[pruned ? ORC_BC_FWD_PRUNED : ORC_BC_FWD_KEPT]++;
+            for (const Nwd &nb : list) trips.push_back(Trip{nb.node, nb.d.d, p}); /* update_back_pointer :720-737 */
+        }
+        std::sort(trips.begin(), trips.end(), [](const Trip &a, const Trip &b) {
+            return a.dst != b.dst ? a.dst < b.dst : a.d != b.d ? a.d < b.d : a.src < b.src;
+        });
+        /* an unlabeled destination cannot already hold a source of this batch: appended as they come; the second
+         * pass of a labeled batch can repeat an edge of the first, so its lists go through the merge */
+        const bool merge = sw.order_by_id && has_labels;
+        for (size_t s = 0; s < trips.size();) {
+            size_t e = s;
+            while (e < trips.size() && trips[e].dst == trips[s].dst) e++;
+            const uint32_t q = trips[s].dst;
+            size_t take = e - s;
+            if (sw.back_src_cap && take > sw.back_src_cap) {
+                take = sw.back_src_cap;
+                bc[ORC_BC_BACK_SRC_CUT]++;
+            }
+            std::vector<Nwd> add;
+            for (size_t i = s; i < s + take; i++) {
+                add.push_back(Nwd{trips[i].src, Dwtb{trips[i].d, ipd(trips[i].src, q)}});
+                for (const Nwd &x : nbrs[q])
+                    if (x.node == trips[i].src) bc[ORC_BC_BACK_REPEAT]++;
+            }
+            bool pruned;
+            add_neighbors(q, add, back_keep, merge, &pruned);
+            bc[pruned ? ORC_BC_BACK_PRUNED : merge ? ORC_BC_BACK_MERGED : ORC_BC_BACK_APPENDED]++;
+            s = e;
+        }
     }
 };
 
@@ -922,4 +1013,52 @@ extern "C" void orc_build(uint32_t n, uint32_t words, const uint64_t *codes, uin
         k++;
     }
     if (out_n_start_labels) *out_n_start_labels = k;
+}
+
+extern "C" void orc_build_batched(uint32_t n, uint32_t words, const uint64_t *codes, uint32_t R,
+                                  uint32_t search_list_size, double max_alpha, int32_t has_labels,
+                                  const uint32_t *label_off, const int16_t *labels, uint32_t max_batch,
+                                  const orc_build_switches *sw, uint32_t *out_nbrs, uint32_t out_stride,
+                                  uint64_t *out_counts) {
+    Builder b;
+    b.n = n;
+    b.words = words;
+    b.R = R;
+    b.L = search_list_size;
+    b.max_alpha = max_alpha;
+    b.has_labels = has_labels != 0;
+    b.codes = codes;
+    b.label_off = label_off;
+    b.labels = labels;
+    b.max_during_build = (size_t)std::ceil((double)R * 1.3);
+    b.nbrs.resize(n);
+    if (sw) b.sw = *sw;
+    if (max_batch == 0) max_batch = 0xFFFFFFFFu;
+    /* node 0 alone (a batch of one is the reference's insert), then batches that grow with the graph */
+    for (uint32_t lo = 0; lo < n;) {
+        const uint32_t m = std::min(std::min(std::max<uint32_t>(1, lo / 16), max_batch), n - lo);
+        for (uint32_t p = lo; p < lo + m; p++) { /* graph/mod.rs:490-533: start nodes, before the node's own search */
+            if (!b.have_start) {
+                b.have_start = true;
+                b.start_default = p;
+            }
+            uint32_t nl;
+            const int16_t *l = b.labs(p, &nl);
+            for (uint32_t i = 0; i < nl; i++)
+                if (!b.start_labeled.count(l[i])) b.start_labeled[l[i]] = p;
+        }
+        if (b.has_labels) b.insert_batch(lo, m, false);
+        b.insert_batch(lo, m, true);
+        lo += m;
+    }
+    for (uint32_t i = 0; i < n; i++) { /* build.rs:905-960 finalize_index_build */
+        std::vector<Nwd> list = b.nbrs[i];
+        if (list.size() > R) {
+            list = b.prune(i, list);
+            b.bc[ORC_BC_FINAL_PRUNED]++;
+        }
+        for (uint32_t j = 0; j < out_stride; j++)
+            out_nbrs[(size_t)i * out_stride + j] = j < list.size() ? list[j].node : ORC_INVALID_NODE;
+    }
+    if (out_counts) std::memcpy(out_counts, b.bc, sizeof b.bc);
 }

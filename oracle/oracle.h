@@ -132,6 +132,53 @@ void orc_build(uint32_t n, uint32_t words, const uint64_t *codes, uint32_t R,
                uint32_t *out_start_label_nodes, uint32_t *out_n_start_labels,
                uint32_t start_label_cap);
 
+/* ---- model of the product's batched builder (dann_build_graph) --------------------------
+ * The SAME prune / add_neighbors / search_for_build as orc_build, run under the batch schedule:
+ * node 0 first, then batches of min(max(1, lo/16), max_batch, n - lo) nodes; every search of a
+ * batch sees the graph as it stood before the batch, then the forward lists are written, then
+ * the back-links of the whole batch are added per destination in (distance, source) order.  A
+ * labeled batch runs twice (filtered, then unfiltered; the second pass merges with the first).
+ * Each way the GPU builder departs from the reference is one switch; all zero and
+ * max_batch == 1 is the reference's serial build (== orc_build). */
+typedef struct {
+    uint32_t scan_ties;     /* 1: the build search orders equal distances as a scan does (tie-break 0,
+                             *    neighbor_with_distance.rs:31-43) instead of by |id - p| (:45-49) */
+    uint32_t order_by_id;   /* 1: prune candidates are ordered by (distance, id) instead of the stable sort by
+                             *    DistanceWithTieBreak, and a list that went through a merge is stored in that order */
+    uint32_t visited_cap;   /* N > 0: only the first N entries of the distance-ordered visited list are handed over */
+    uint32_t cand_cap;      /* N > 0: a forward prune sees its current neighbours + the closest N - deg visited nodes */
+    uint32_t back_src_cap;  /* N > 0: a destination takes at most the N closest new sources of one batch */
+    uint32_t slots;         /* N > 0: lists have N storage slots: back-links overflow at min(N, ceil(1.3 R)) */
+    uint32_t fwd_keep_slots; /* 1: a forward list is pruned only when it outgrows `slots`, not ceil(1.3 R) */
+} orc_build_switches;
+
+/* how often each branch ran (indices into out_counts[ORC_BC_N]) */
+enum {
+    ORC_BC_FWD_KEPT = 0,     /* forward list written unpruned */
+    ORC_BC_FWD_PRUNED,       /* forward list pruned to R */
+    ORC_BC_FWD_MERGED,       /* forward pass that started from a non-empty list (second pass of a labeled insert) */
+    ORC_BC_BACK_APPENDED,    /* back-links appended, no merge */
+    ORC_BC_BACK_MERGED,      /* back-links merged and stored in candidate order, no prune */
+    ORC_BC_BACK_PRUNED,      /* back-link overflow: pruned to R */
+    ORC_BC_BACK_SRC_CUT,     /* destination with more than back_src_cap new sources in one batch */
+    ORC_BC_BACK_REPEAT,      /* a new source that was already a neighbour of its destination */
+    ORC_BC_FINAL_PRUNED,     /* finalize: list longer than R pruned */
+    ORC_BC_VISITED_CUT,      /* visited list longer than visited_cap */
+    ORC_BC_CAND_CUT,         /* visited nodes dropped by cand_cap */
+    ORC_BC_EMPTY_SEARCH,     /* a search that visited nothing (no start node for any label of the point) */
+    ORC_BC_ROUND2_KEPT,      /* prune: a neighbour accepted in the second alpha round */
+    ORC_BC_TIE_FACTOR,       /* prune: the |id - p| / |id - kept| factor of two zero distances */
+    ORC_BC_ZERO_OCCLUDED,    /* prune: zero distance to the kept neighbour, non-zero to the point */
+    ORC_BC_LABEL_SKIP,       /* prune: occlusion skipped by contains_intersection */
+    ORC_BC_N
+};
+
+void orc_build_batched(uint32_t n, uint32_t words, const uint64_t *codes, uint32_t R,
+                       uint32_t search_list_size, double max_alpha, int32_t has_labels,
+                       const uint32_t *label_off, const int16_t *labels, uint32_t max_batch /* 0 = unbounded */,
+                       const orc_build_switches *sw, uint32_t *out_nbrs /* [n * out_stride], INVALID-padded */,
+                       uint32_t out_stride /* >= R */, uint64_t *out_counts /* [ORC_BC_N] or NULL */);
+
 #ifdef __cplusplus
 }
 #endif

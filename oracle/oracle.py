@@ -183,6 +183,43 @@ def build_graph(codes, R: int, search_list_size: int = 100, max_alpha: float = 1
     return nbrs, int(sd.value), sl[:k].copy(), sn[:k].copy()
 
 
+class _BuildSwitches(C.Structure):
+    _fields_ = [(k, C.c_uint32) for k in ("scan_ties", "order_by_id", "visited_cap", "cand_cap", "back_src_cap", "slots",
+                                          "fwd_keep_slots")]
+
+
+# dann_build_graph's departures from the reference's build rules, by name (oracle.h orc_build_switches; DESIGN.md 6b)
+GPU_BUILDER_SWITCHES = dict(scan_ties=1, order_by_id=1, visited_cap=256, cand_cap=128, back_src_cap=64, slots=64,
+                            fwd_keep_slots=1)
+
+BUILD_COUNTERS = ("fwd_kept", "fwd_pruned", "fwd_merged", "back_appended", "back_merged", "back_pruned", "back_src_cut",
+                  "back_repeat", "final_pruned", "visited_cut", "cand_cut", "empty_search", "round2_kept", "tie_factor",
+                  "zero_occluded", "label_skip")
+
+
+def build_graph_batched(codes, R: int, search_list_size: int = 100, max_alpha: float = 1.2, label_off=None, labels=None,
+                        max_batch: int = 0, switches=None, stride=None):
+    """The model of the batched builder: orc_build's own prune / add_neighbors / search under the batch schedule, with
+    the named `switches` (a dict; None = the reference's rules).  -> nbrs[n, stride] (INVALID-padded), branch counts"""
+    codes = np.ascontiguousarray(codes, dtype=np.uint64)
+    n, words = codes.shape
+    stride = R if stride is None else stride
+    has_labels = label_off is not None
+    if has_labels:
+        label_off = np.ascontiguousarray(label_off, dtype=np.uint32)
+        labels = np.ascontiguousarray(labels, dtype=np.int16)
+    sw = _BuildSwitches(**(switches or {}))
+    nbrs = np.full((n, stride), INVALID_NODE, np.uint32)
+    counts = np.zeros(len(BUILD_COUNTERS), np.uint64)
+    fn = lib().orc_build_batched
+    fn.restype = None
+    fn.argtypes = [C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint32, C.c_uint32, C.c_double, C.c_int32, C.c_void_p,
+                   C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
+    fn(n, words, _p(codes), R, search_list_size, max_alpha, int(has_labels), _p(label_off) if has_labels else None,
+       _p(labels) if has_labels else None, min(int(max_batch), 0xFFFFFFFF), C.addressof(sw), _p(nbrs), stride, _p(counts))
+    return nbrs, dict(zip(BUILD_COUNTERS, (int(c) for c in counts)))
+
+
 @dataclass
 class _Keep:
     arrays: list

@@ -38,7 +38,7 @@ __device__ __forceinline__ bool labels_contains_intersection(const int16_t *c, u
 }
 
 #define DANN_BUILD_CMAX 128u /* candidates considered by one prune */
-#define DANN_BUILD_SLACK 64u /* neighbour slots per node while building (the reference: ceil(1.3 R)) */
+#define DANN_BUILD_SLACK 64u /* neighbour slots per node while building (the reference keeps up to ceil(1.3 R), unbounded by slots) */
 
 /* candidate key: (distance << 32) | node id ; sorted ascending = reference's candidates.sort() up to
  * the tie-break among equal distances (id order here, ip_distance order there) */
@@ -214,7 +214,10 @@ __global__ void __launch_bounds__(256) dann_build_prune_kernel(BuildArgs a, uint
             __syncwarp();
         }
         uint32_t cnt;
-        if (C <= DANN_BUILD_SLACK) { /* not more than max_neighbors_during_build: keep them all */
+        /* a forward list keeps every candidate the 64 slots hold until a back-link or finalize prunes it - NOT the
+         * reference's max_neighbors_during_build = ceil(1.3 R) that back-links overflow at (a.limit): a new node keeps
+         * more out-edges while its batch mates cannot see it yet.  Equal at R >= 50 (min(64, 65)); DESIGN.md 6b */
+        if (C <= DANN_BUILD_SLACK) {
             for (uint32_t t = lane; t < C; t += 32) {
                 oid[t] = (uint32_t)ck[t];
                 od[t] = (uint16_t)(ck[t] >> 32);

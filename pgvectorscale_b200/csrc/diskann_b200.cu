@@ -717,6 +717,9 @@ static int run_search(dann_index *ix, const uint64_t *d_q_codes, const int16_t *
         SearchPlan p;
         rc = make_plan(ix, nq, L, c_target, grow, d_label_off != nullptr, &p, false, vis_out == nullptr);
         if (rc) return rc;
+        if (vis_out && !p.pairs) /* dann_search.cuh has no build mode: its launch would leave vis_out_len unwritten */
+            return fail(DANN_ERR_STATE, "build mode needs the two-warp search kernel, which alone hands over its visited list: "
+                                        "unset DANN_SEARCH_KERNEL=1");
         const size_t slots = (size_t)p.grid * p.W;
         if (!p.bitmap_words) CK(ix->ws_hash.reserve(slots * p.hash_cap * sizeof(uint32_t)));
         if (!p.lean) CK(ix->ws_cand.reserve(slots * p.cand_cap * sizeof(uint32_t))); /* lean entries carry their node */
@@ -1041,6 +1044,13 @@ extern "C" int dann_build_graph(dann_index *ix, int num_neighbors, int search_li
     const uint32_t n = v.n;
     const uint32_t vis_cap = 2 * DANN_BUILD_CMAX;
     const uint32_t mb = std::min<uint32_t>(max_batch, n);
+    /* a prune warp stages its 128 candidate codes in shared memory (row stride cw | 1): checked before anything is
+     * allocated or the neighbour rows are reset, so a refused build leaves the index as it was */
+    const size_t pw = ((size_t)DANN_BUILD_CMAX * 8 + (size_t)DANN_BUILD_CMAX * (v.cw | 1u) * 8 + DANN_BUILD_CMAX * 4 +
+                       DANN_BUILD_SLACK * 4 + DANN_BUILD_SLACK * 2 + 15) & ~(size_t)15;
+    const size_t budget = ix->smem_optin > 1024 ? ix->smem_optin - 1024 : ix->smem_optin;
+    const int bw = (int)std::min<size_t>(8, budget / pw);
+    if (bw < 1) return fail(DANN_ERR_CAPACITY, "SBQ code of %u words is too wide for the prune kernel's shared memory", v.words);
 
     DevBuf b_dist, b_deg, b_vis, b_vlen, b_k0, b_k1, b_v0, b_v1, b_heads, b_tmp, b_stream, b_slen, b_stats;
     struct Cleanup {
@@ -1085,12 +1095,7 @@ extern "C" int dann_build_graph(dann_index *ix, int num_neighbors, int search_li
     ba.max_alpha = max_alpha;
     ba.label_off = v.has_labels ? v.label_off : nullptr;
     ba.labels = v.has_labels ? v.labels : nullptr;
-    const size_t pw = ((size_t)DANN_BUILD_CMAX * 8 + (size_t)DANN_BUILD_CMAX * ba.cws * 8 + DANN_BUILD_CMAX * 4 +
-                       DANN_BUILD_SLACK * 4 + DANN_BUILD_SLACK * 2 + 15) & ~(size_t)15;
     ba.per_warp_smem = (uint32_t)pw;
-    const size_t budget = ix->smem_optin > 1024 ? ix->smem_optin - 1024 : ix->smem_optin;
-    int bw = (int)std::min<size_t>(8, budget / pw);
-    if (bw < 1) return fail(DANN_ERR_CAPACITY, "SBQ code of %u words is too wide for the prune kernel's shared memory", v.words);
     const size_t bsmem = pw * bw + DANN_SMEM_SLACK;
     CK(cudaFuncSetAttribute(dann_build_prune_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bsmem));
     CK(cudaFuncSetAttribute(dann_build_backlink_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bsmem));

@@ -285,6 +285,45 @@ def test_small_accuracy_connectivity_property(train_on_data):
     assert len(r["tid"]) == 1000 and len(set(r["tid"].tolist())) == 1000
 
 
+# ---- the model of the batched builder is the serial restatement when nothing departs from it ----
+@pytest.mark.parametrize("n,dim,kind,labels,R,L", [
+    (1, 8, "normal", False, 4, 4), (2, 8, "normal", True, 4, 4), (400, 16, "normal", False, 10, 20),
+    (600, 2, "uniform", False, 10, 10),      # tie-heavy: the stable sort by DistanceWithTieBreak, the tie factor
+    (400, 24, "normal", True, 8, 20),        # both passes of a labeled insert, contains_intersection
+    (300, 40, "normal", False, 50, 100)])    # max_neighbors_during_build = 65: lists longer than 64
+def test_batched_build_model_with_no_switch_and_batches_of_one_is_the_serial_build(n, dim, kind, labels, R, L):
+    """oracle.build_graph_batched runs orc_build's own prune / add_neighbors / search_for_build under the GPU builder's
+    schedule (tests/test_zz_o_build_model_gpu.py compares dann_build_graph with it).  With every departure switched off
+    and max_batch = 1 that schedule is the reference's serial insert: the neighbour arrays are identical."""
+    s = build_case(n, dim, L2, seed=3, kind=kind, R=R, L_build=L, labels=labels)
+    nb, counts = oracle.build_graph_batched(s.codes, R, L, 1.2, s.label_off if labels else None,
+                                            s.labels if labels else None, max_batch=1)
+    assert np.array_equal(nb, s.nbrs)
+    assert n < 100 or (counts["back_pruned"] and counts["final_pruned"])
+    if kind == "uniform":
+        assert counts["tie_factor"] and counts["zero_occluded"]
+    if labels and n > 100:
+        assert counts["fwd_merged"] and counts["back_repeat"] and counts["label_skip"]
+
+
+def test_batched_build_model_switches_each_change_the_graph():
+    """Every named departure is live: switching it on alone moves at least one edge of a build that exercises it."""
+    s = build_case(1500, 2, L2, seed=5, kind="uniform", R=10, L_build=10)
+    s2 = build_case(1200, 32, L2, seed=11, kind="normal", R=16, L_build=150)
+    for code, R, L in ((s.codes, 10, 10), (s2.codes, 16, 300)):
+        base, _ = oracle.build_graph_batched(code, R, L, 1.2, max_batch=0)
+        moved = {k: not np.array_equal(base, oracle.build_graph_batched(code, R, L, 1.2, max_batch=0, switches={k: v})[0])
+                 for k, v in (("scan_ties", 1), ("order_by_id", 1), ("visited_cap", 256), ("cand_cap", 128),
+                              ("back_src_cap", 64), ("slots", 12))}
+        if L == 10:
+            assert moved["scan_ties"] and moved["order_by_id"] and moved["slots"], moved
+        else:
+            assert moved["visited_cap"] and moved["cand_cap"], moved
+    a = oracle.build_graph_batched(s2.codes, 16, 150, 1.2, max_batch=0, switches=dict(slots=64))[0]
+    b = oracle.build_graph_batched(s2.codes, 16, 150, 1.2, max_batch=0, switches=dict(slots=64, fwd_keep_slots=1))[0]
+    assert not np.array_equal(a, b)
+
+
 # ---- the two restatements agree on whole scans ---------------------------------------------
 @pytest.mark.parametrize("dist,bits,labels,dim_index", [(COSINE, 2, False, None), (L2, 1, False, None),
                                                         (IP, 2, True, None), (COSINE, 2, True, 40)])

@@ -108,8 +108,9 @@ def test_small_built_labeled_graph_valid_and_parity(lib):
         idx.close()
 
 
-# floors leave room for the builder's run-to-run variation on hardware (atomics order); under emulation the five cases
-# return 997, 446, 1000, 1000 and 750 of 1000 rows
+# floors leave room for the rescue's run-to-run variation on hardware (its kernels race by design; without it the
+# build is deterministic, tests/test_zz_o_build_model_gpu.py); under emulation the five cases return 997, 446, 1000, 1000
+# and 750 of 1000 rows
 @pytest.mark.parametrize("dim,R,rescue,floor", [(8, 10, 0, 0.98), (2, 10, 0, 0.3), (8, 10, 1, 0.995), (2, 20, 1, 0.99),
                                                  (2, 10, 1, 0.6)])
 def test_small_accuracy_connectivity_of_the_gpu_builder(lib, monkeypatch, dim, R, rescue, floor):
