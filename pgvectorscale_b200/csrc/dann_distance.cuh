@@ -77,9 +77,14 @@ __device__ __forceinline__ float full_distance_group8(int type, const float *__r
             dist = __fadd_rn(dist, __fmul_rn(xi, yi));
         }
     }
-    if (type == DANN_L2) return dist;                 /* distance/mod.rs:88-104 (no sqrt) */
-    if (type == DANN_IP) return -dist;                /* :175-190 */
-    float r = __fsub_rn(1.0f, dist);                  /* distance_x86.rs:34-36 (1.0 - ip).max(0.0) */
+    /* A NaN sum (inf + -inf; finite inputs reach it only in an inner product) carries the bits of the reference's x86
+     * build: SSE's default NaN 0xFFC00000, sign-flipped by the inner product's `-dist`.  The GPU's float unit would
+     * return its own canonical NaN (0x7FFFFFFF), so the constant is selected, not computed: any float operation on it
+     * would canonicalise it again. */
+    const bool nan = dist != dist;
+    if (type == DANN_L2) return nan ? __int_as_float(0xFFC00000) : dist;  /* distance/mod.rs:88-104 (no sqrt) */
+    if (type == DANN_IP) return nan ? __int_as_float(0x7FC00000) : -dist; /* :175-190 */
+    float r = __fsub_rn(1.0f, dist);                  /* distance_x86.rs:34-36 (1.0 - ip).max(0.0): NaN -> +0.0 */
     return r > 0.0f ? r : 0.0f;
 }
 

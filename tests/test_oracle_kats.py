@@ -177,6 +177,140 @@ def test_quantizer_matches_python_restatement():
             assert [int(x) for x in a] == b
 
 
+# ---- values the uniform / Gaussian fixtures never produce (tests/test_zz_p_values_gpu.py) -----------------------------
+def _bits(x):
+    return int(np.float32(x).view(np.uint32))
+
+
+def _value_cases():
+    """(name, kind, x, y, expected bits or a predicate) at a tail-only, a body + tail and a body-only length."""
+    f = np.float32
+    out = []
+    for n in (7, 40, 96):
+        z = np.zeros(n, f)
+        x, y = z.copy(), z.copy()
+        # x86: inf + -inf = 0xFFC00000, and the inner product's `-dist` flips it to 0x7FC00000
+        x[0] = y[0] = x[1] = f(3e38)
+        y[1] = f(-3e38)
+        if n >= 32:
+            x[1] = y[1] = 0.0
+            x[8] = y[0] = x[0] = f(3e38)
+            y[8] = f(-3e38)
+        out += [("nan", IP, x, y, 0x7FC00000), ("nan-cos", COSINE, x, y, 0)]
+        x, y = z.copy(), z.copy()
+        x[0], y[0], x[n - 1], y[n - 1] = f(3e38), f(3e38), f(-3e38), f(-3e38)
+        out += [("inf", IP, x, y, 0xFF800000), ("inf-l2", L2, x, -y, 0x7F800000), ("equal-l2", L2, x, x, 0)]
+        x = np.full(n, f(1e-20))
+        h = np.full(n, f(5e-21))
+        out += [("subnormal-ip", IP, x, x, lambda b: 0x80000000 < b < 0x80800000),
+                ("subnormal-l2", L2, h, -h, lambda b: 0 < b < 0x00800000),
+                ("denormal-in", IP, np.full(n, f(1e-40)), np.full(n, f(0.5)), lambda b: 0x80000000 < b < 0x80800000)]
+        x, y = z.copy(), z.copy()
+        x[0], y[n - 1] = 1.0, -1.0
+        out += [("orthogonal-ip", IP, x, y, 0x80000000), ("orthogonal-cos", COSINE, x, y, _bits(1.0)),
+                ("neg-zeros-ip", IP, np.full(n, f(-0.0)), z, 0x80000000), ("self-cos", COSINE, x, x, 0)]
+    return out
+
+
+@pytest.mark.parametrize("case", range(len(_value_cases())))
+def test_distance_bits_on_nan_inf_subnormal_and_signed_zero_inputs(case):
+    """The scalar restatement, the real AVX2 build and the Python restatement give the same bits, and the bits the
+    x86 reference gives: NaN inner products 0x7FC00000, +-inf, subnormal sums kept, -0.0 for an exactly zero product."""
+    name, kind, x, y, want = _value_cases()[case]
+    with np.errstate(all="ignore"):
+        got = {impl: _bits(oracle.distance(kind, x, y, impl)) for impl in ("emu", "avx2")}
+        got["pyref"] = _bits(pyref.distance(kind, x, y))
+    assert len(set(got.values())) == 1, (name, {k: hex(v) for k, v in got.items()})
+    b = got["avx2"]
+    assert want(b) if callable(want) else b == want, (name, len(x), hex(b))
+
+
+def test_preprocess_cosine_of_overflowing_and_subnormal_rows():
+    """A norm that overflows divides every component by +inf: the row becomes signed zeros.  A norm below f32::EPSILON
+    (subnormal or underflowed to zero) leaves the row untouched."""
+    f = np.float32
+    rows = {"3e38": np.array([3e38, 1.0, -2.0, 0.5, -0.0], f), "1e20": np.full(40, f(1e20)),
+            "-1e20": np.full(40, f(-1e20)), "1e-40": np.array([1e-40, -1e-40, 0.0, -0.0, 3e-39], f),
+            "1e-20": np.full(40, f(1e-20))}
+    for name, v in rows.items():
+        with np.errstate(all="ignore"):
+            a, b = oracle.preprocess_cosine(v), pyref.preprocess_cosine(v)
+        assert np.array_equal(a.view(np.uint32), b.view(np.uint32)), name
+        if name.endswith("e20") or name == "3e38":
+            assert not a.any() and np.array_equal(np.signbit(a), np.signbit(v)), name
+        else:
+            assert np.array_equal(a.view(np.uint32), v.view(np.uint32)), name
+
+
+def test_quantizer_edges_match_python_restatement():
+    """Constant columns (m2 = 0: z = +-inf, or NaN at the mean), +-0 means, count 0 / 1 / 2^24 + 3 / 2^53 + 1, query
+    components on every bucket edge and its nextafter neighbours: the fixtures of tests/test_zz_p_values_gpu.py."""
+    from test_zz_p_values_gpu import COUNTS, quantizer_case
+    for count in COUNTS:
+        for bits in (1, 2, 3, 4):
+            s, q, _, _ = quantizer_case(count, bits)
+            for r in q:
+                with np.errstate(all="ignore"):
+                    want = pyref.quantize(r, bits, s.mean, s.m2, count, s.words)
+                assert [int(x) for x in oracle.quantize(r, bits, s.mean, s.m2, count)] == want, (count, bits)
+    # hand-worked: count 0 (std = +inf, z = 0, index = ranges / 2), a constant column, `count as f32` to nearest
+    one = np.ones(1, np.float32)
+    assert int(oracle.quantize(np.array([5.0], np.float32), 3, 0 * one, one, 0)[0]) == 0b011       # index 2.0
+    assert int(oracle.quantize(np.array([5.0], np.float32), 2, 0 * one, one, 0)[0]) == 0b01        # index 1.5
+    assert [int(oracle.quantize(np.array([v], np.float32), 4, one, 0 * one, 7)[0]) for v in (2.0, 1.0, 0.0)] == \
+        [0b1111, 0, 0]
+    # count 2^24 + 3 converts to 2^24 + 4 = m2: variance 1, z = 1, index (1 + 2) / (4 / 3) = 2.2499998 -> 2 ones
+    m2 = np.array([16777220.0], np.float32)
+    assert int(oracle.quantize(np.array([1.0], np.float32), 2, 0 * one, m2, (1 << 24) + 3)[0]) == 0b11
+
+
+@pytest.mark.parametrize("bits", [3, 4, 5, 7, 8, 16, 31, 32])
+def test_quantizer_wide_bits_match_python_restatement(bits):
+    """3 to 32 bits per dimension, trained on data, at 13 dimensions (a dimension's bits straddle a word unless
+    64 % bits == 0), rows far past the last edge included."""
+    rng = np.random.default_rng(bits)
+    data = rng.standard_normal((60, 13)).astype(np.float32)
+    mean, m2, count = oracle.train(data, bits)
+    rows = np.concatenate([data[:10], 4 * data[10:12], np.zeros((1, 13), np.float32)])
+    full = 0
+    for r in rows:
+        a = oracle.quantize(r, bits, mean, m2, count)
+        assert [int(x) for x in a] == pyref.quantize(r, bits, mean, m2, count, len(a))
+        full += sum(bin(int(w)).count("1") for w in a)
+    assert full > 13 * bits
+
+
+@pytest.mark.parametrize("family", ["duplicates", "overflow"])
+def test_cpp_oracle_equals_python_restatement_on_ties_and_overflow(family):
+    """Whole scans on 160 rows drawn from 9 distinct vectors (cosine, L2: zero distances and runs of equal exact
+    distances in the rerank window) and on rows with +-3e38 components (inner product: +-inf and NaN distances)."""
+    from test_zz_p_values_gpu import duplicate_rows, overflow_rows, trained_index
+    if family == "duplicates":
+        v, q = duplicate_rows(160, 24, 9, 5, "normal")
+        cases = [(trained_index(v, COSINE, 2, R=12, L_build=24), q[[0, 1, 13, 24]]),
+                 (trained_index(v, L2, 1, R=12, L_build=24), q[[2, 14, 24]])]
+    else:
+        v, q = overflow_rows(160, 40, 7)
+        cases = [(trained_index(v, IP, 2, R=12, L_build=24), q[[0, 8, 10, 16]]),
+                 (trained_index(v, L2, 2, R=12, L_build=24), q[[1, 9, 11]])]
+    special = 0
+    for s, qs in cases:
+        for qi in qs:
+            for (L, rescore, rows) in ((20, 10, 15), (40, 60, 30)):
+                with np.errstate(all="ignore"):
+                    a = oracle.scan(s, qi, None, L, rescore, rows)
+                    b_rows, b_stats = pyref.scan(s, qi, None, L, rescore, rows)
+                assert a["tid"].tolist() == [r[0] for r in b_rows]
+                assert a["node"].tolist() == [r[1] for r in b_rows]
+                assert a["dist"].view(np.uint32).tolist() == \
+                    np.array([r[2] for r in b_rows], np.float32).view(np.uint32).tolist()
+                assert a["stats"] == b_stats
+                d = a["dist"]
+                special += int((d == 0).sum() + (d[1:] == d[:-1]).sum()) if family == "duplicates" else \
+                    int(np.isnan(d).sum() + np.isinf(d).sum())
+    assert special > 20, special
+
+
 # ---- reference SQL KATs restated (index created BEFORE the inserts => zero means) -----------
 def _three_vector_index(dist):
     v = np.array([[1, 1, 1], [2, 2, 2], [3, 3, 3]], np.float32)
