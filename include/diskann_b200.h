@@ -237,6 +237,32 @@ int dann_group_search_batch(dann_group *g, const float *queries, const int16_t *
                             uint32_t *out_count, dann_query_stats *out_stats);
 void dann_group_free(dann_group *g);
 
+/* ---- a table split into shards: one independent index per shard, one merged top-k per query -------------------
+ * Shard i is an ordinary diskann index over a disjoint set of the table's rows (its own graph, SBQ means and start
+ * nodes), loaded on devices[i] (NULL: device i); several shards may share a device.  1..256 shards, which must agree
+ * on dim, dim_index, distance_type and has_labels (else DANN_ERR_INVALID_ARG); they may differ in n (0 included),
+ * bits, means and R.  A failed load frees the shards loaded so far.  Plain-layout shards are not supported.
+ *
+ * dann_shards_search_batch runs every shard's host-buffer batch on all B queries (one worker thread per distinct
+ * device, that device's shards in shard order: each shard's rows, distance bits and counters are what a private
+ * dann_search_batch on it gives), then merges them on the device of shard 0.  The merge is a k-way merge of the
+ * shards' lists by their heads: k times, among the shards whose list of count_s[b] rows is not used up, take the head
+ * with the smallest (f32::total_cmp key of its distance, shard index) and advance that shard.  A shard's rows
+ * therefore appear as a prefix of its own list, in its own order; one shard gives exactly dann_search_batch's rows.
+ * out_tid / out_dist / out_shard [B*k] (DANN_INVALID_TID, NaN and -1 past out_count[b]), out_count [B] =
+ * min(k, sum of the shards' counts), out_stats [nshards*B] shard-major (query b of shard s at s*B + b); any may be
+ * NULL except out_tid.  rescore == 0 is DANN_ERR_INVALID_ARG (rows would carry no distance to merge on); a shard's own
+ * failure fails the call as "shard i: ...".  One call at a time per handle. */
+typedef struct dann_shards dann_shards;
+int dann_shards_create(const dann_snapshot_desc *const *shards, int nshards, const int *devices, dann_shards **out);
+int dann_shards_count(const dann_shards *g);
+dann_index *dann_shards_index(dann_shards *g, int i); /* borrowed: build a shard's graph / attach its rows in place; NULL if out of range */
+int dann_shards_search_batch(dann_shards *g, const float *queries, const int16_t *labels, const int32_t *label_off,
+                             int B, int k, int search_list_size, int rescore,
+                             uint64_t *out_tid, float *out_dist, int32_t *out_shard, uint32_t *out_count,
+                             dann_query_stats *out_stats);
+void dann_shards_free(dann_shards *g);
+
 /* ---- reading an index RELATION FILE (SURVEY.md §8f row 2; pgvectorscale_b200/csrc/dann_pgreader.h) -------------------
  * Host-only, no GPU involved.  Replaces, for an external loader (the sidecar after a CHECKPOINT, an offline exporter):
  *   ReadablePage::read / get_type / get_item_unchecked   util/page.rs:254-290   dann_pg_relation_open / _info

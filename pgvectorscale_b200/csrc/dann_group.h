@@ -10,56 +10,47 @@
 #include <condition_variable>
 #include <thread>
 
-struct GroupWorker {
-    dann_index *ix = nullptr;
-    std::thread th;
-    /* the slice of the current call */
-    int lo = 0, hi = 0;
-    int rc = 0;
-    std::string err;
-    uint64_t seen = 0; /* generation this worker has finished */
-};
-
-struct dann_group {
-    std::vector<GroupWorker> w;
-    std::mutex mu, call_mu; /* call_mu: one batch call at a time per group */
+/* One host thread per worker, driven by generations: each call publishes its arguments, bumps `gen` and waits until
+ * every worker has run job(i) for that generation.  dann_group (one worker per replica) and dann_shards (one worker per
+ * distinct device) both run on it. */
+struct WorkerLoop {
+    struct Worker {
+        std::thread th;
+        int rc = 0;
+        std::string err;
+        uint64_t seen = 0; /* generation this worker has finished */
+    };
+    std::vector<Worker> w;
+    std::mutex mu;
     std::condition_variable cv_go, cv_done;
     uint64_t gen = 0;
     bool stop = false;
-    /* arguments of the current call (borrowed from the caller for its duration) */
-    const float *queries = nullptr;
-    const int16_t *labels = nullptr;
-    const int32_t *label_off = nullptr;
-    int k = 0, L = 0, rescore = 0;
-    uint32_t dim = 0;
-    uint64_t *out_tid = nullptr;
-    float *out_dist = nullptr;
-    uint32_t *out_count = nullptr;
-    dann_query_stats *out_stats = nullptr;
+    std::function<int(size_t)> job; /* the work of worker i in the current generation; its error text is g_err */
+
+    void start(size_t n, std::function<int(size_t)> fn) {
+        job = std::move(fn);
+        w.resize(n);
+        for (size_t i = 0; i < n; i++) w[i].th = std::thread([this, i] { run(i); });
+    }
 
     void run(size_t i) {
-        GroupWorker &me = w[i];
+        Worker &me = w[i];
         uint64_t done = 0;
         std::unique_lock<std::mutex> lk(mu);
         for (;;) {
             cv_go.wait(lk, [&] { return stop || gen != done; });
             if (stop) return;
             const uint64_t g = gen;
-            const int lo = me.lo, hi = me.hi;
             lk.unlock();
             int rc = DANN_OK;
             std::string err;
-            if (hi > lo) {
-                try {
-                    rc = search_batch_host(me.ix, queries + (size_t)lo * dim, labels, label_off ? label_off + lo : nullptr, hi - lo,
-                                           k, L, rescore, out_tid + (size_t)lo * k, out_dist ? out_dist + (size_t)lo * k : nullptr,
-                                           nullptr, out_count ? out_count + lo : nullptr, out_stats ? out_stats + lo : nullptr);
-                    if (rc) err = g_err; /* thread-local message of this worker */
-                } catch (const std::bad_alloc &) {
-                    rc = DANN_ERR_OOM;
-                } catch (...) {
-                    rc = DANN_ERR_STATE;
-                }
+            try {
+                rc = job(i);
+                if (rc) err = g_err; /* thread-local message of this worker */
+            } catch (const std::bad_alloc &) {
+                rc = DANN_ERR_OOM;
+            } catch (...) {
+                rc = DANN_ERR_STATE;
             }
             lk.lock();
             me.rc = rc;
@@ -71,6 +62,53 @@ struct dann_group {
             me.seen = g;
             cv_done.notify_all();
         }
+    }
+
+    /* runs one generation; the caller has published the call's arguments (they are read after `mu` is taken) */
+    void call() {
+        std::unique_lock<std::mutex> lk(mu);
+        const uint64_t g = ++gen;
+        cv_go.notify_all();
+        cv_done.wait(lk, [&] {
+            for (const Worker &x : w)
+                if (x.seen != g) return false;
+            return true;
+        });
+    }
+
+    void shutdown() {
+        {
+            std::lock_guard<std::mutex> lk(mu);
+            stop = true;
+        }
+        cv_go.notify_all();
+        for (Worker &x : w)
+            if (x.th.joinable()) x.th.join();
+    }
+};
+
+struct dann_group {
+    std::vector<dann_index *> ix;
+    std::vector<int> lo, hi; /* each replica's slice of the current call */
+    WorkerLoop loop;
+    std::mutex call_mu; /* one batch call at a time per group */
+    /* arguments of the current call (borrowed from the caller for its duration) */
+    const float *queries = nullptr;
+    const int16_t *labels = nullptr;
+    const int32_t *label_off = nullptr;
+    int k = 0, L = 0, rescore = 0;
+    uint32_t dim = 0;
+    uint64_t *out_tid = nullptr;
+    float *out_dist = nullptr;
+    uint32_t *out_count = nullptr;
+    dann_query_stats *out_stats = nullptr;
+
+    int run(size_t i) {
+        const int l = lo[i], h = hi[i];
+        if (h <= l) return DANN_OK;
+        return search_batch_host(ix[i], queries + (size_t)l * dim, labels, label_off ? label_off + l : nullptr, h - l, k, L,
+                                 rescore, out_tid + (size_t)l * k, out_dist ? out_dist + (size_t)l * k : nullptr, nullptr,
+                                 out_count ? out_count + l : nullptr, out_stats ? out_stats + l : nullptr);
     }
 };
 
@@ -84,40 +122,36 @@ static void group_bounds(int total, int world, int r, int *lo, int *hi) {
 
 extern "C" void dann_group_free(dann_group *g) {
     if (!g) return;
-    {
-        std::lock_guard<std::mutex> lk(g->mu);
-        g->stop = true;
-    }
-    g->cv_go.notify_all();
-    for (GroupWorker &x : g->w)
-        if (x.th.joinable()) x.th.join();
-    for (GroupWorker &x : g->w) dann_index_free(x.ix);
+    g->loop.shutdown();
+    for (dann_index *x : g->ix) dann_index_free(x);
     delete g;
 }
 
 extern "C" int dann_group_create(const dann_snapshot_desc *snap, int ndev, const int *devices, dann_group **out) try {
     if (!snap || !out || ndev < 1 || ndev > 64) return fail(DANN_ERR_INVALID_ARG, "dann_group_create: bad argument");
     dann_group *g = new dann_group();
-    g->w.resize((size_t)ndev);
+    g->ix.assign((size_t)ndev, nullptr);
+    g->lo.assign((size_t)ndev, 0);
+    g->hi.assign((size_t)ndev, 0);
     for (int i = 0; i < ndev; i++) {
         const int dev = devices ? devices[i] : i;
-        int rc = dann_index_load(snap, dev, &g->w[(size_t)i].ix);
+        int rc = dann_index_load(snap, dev, &g->ix[(size_t)i]);
         if (rc) {
             const std::string keep = g_err;
             dann_group_free(g); /* frees the replicas loaded so far */
             return fail(rc, "dann_group_create: replica %d (device %d): %s", i, dev, keep.c_str());
         }
     }
-    g->dim = g->w[0].ix->v.dim;
-    for (size_t i = 0; i < g->w.size(); i++) g->w[i].th = std::thread([g, i] { g->run(i); });
+    g->dim = g->ix[0]->v.dim;
+    g->loop.start(g->ix.size(), [g](size_t i) { return g->run(i); });
     *out = g;
     return DANN_OK;
 } DANN_CATCH
 
-extern "C" int dann_group_size(const dann_group *g) { return g ? (int)g->w.size() : 0; }
+extern "C" int dann_group_size(const dann_group *g) { return g ? (int)g->ix.size() : 0; }
 
 extern "C" dann_index *dann_group_replica(dann_group *g, int i) {
-    return (g && i >= 0 && (size_t)i < g->w.size()) ? g->w[(size_t)i].ix : nullptr;
+    return (g && i >= 0 && (size_t)i < g->ix.size()) ? g->ix[(size_t)i] : nullptr;
 }
 
 extern "C" int dann_group_search_batch(dann_group *g, const float *queries, const int16_t *labels, const int32_t *label_off,
@@ -125,7 +159,6 @@ extern "C" int dann_group_search_batch(dann_group *g, const float *queries, cons
                                        uint32_t *out_count, dann_query_stats *out_stats) try {
     if (!g || B <= 0 || k <= 0 || !queries || !out_tid) return fail(DANN_ERR_INVALID_ARG, "dann_group_search_batch: bad argument");
     std::lock_guard<std::mutex> one(g->call_mu);
-    std::unique_lock<std::mutex> lk(g->mu);
     g->queries = queries;
     g->labels = labels;
     g->label_off = label_off;
@@ -136,16 +169,10 @@ extern "C" int dann_group_search_batch(dann_group *g, const float *queries, cons
     g->out_dist = out_dist;
     g->out_count = out_count;
     g->out_stats = out_stats;
-    const int world = (int)g->w.size();
-    for (int r = 0; r < world; r++) group_bounds(B, world, r, &g->w[(size_t)r].lo, &g->w[(size_t)r].hi);
-    const uint64_t gen = ++g->gen;
-    g->cv_go.notify_all();
-    g->cv_done.wait(lk, [&] {
-        for (const GroupWorker &x : g->w)
-            if (x.seen != gen) return false;
-        return true;
-    });
+    const int world = (int)g->ix.size();
+    for (int r = 0; r < world; r++) group_bounds(B, world, r, &g->lo[(size_t)r], &g->hi[(size_t)r]);
+    g->loop.call();
     for (int r = 0; r < world; r++)
-        if (g->w[(size_t)r].rc) return fail(g->w[(size_t)r].rc, "replica %d: %s", r, g->w[(size_t)r].err.c_str());
+        if (g->loop.w[(size_t)r].rc) return fail(g->loop.w[(size_t)r].rc, "replica %d: %s", r, g->loop.w[(size_t)r].err.c_str());
     return DANN_OK;
 } DANN_CATCH

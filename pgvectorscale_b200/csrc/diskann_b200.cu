@@ -24,6 +24,7 @@
 #include "dann_search2.cuh"
 #include "dann_search3.cuh"
 #include "dann_build.cuh"
+#include "dann_shards.cuh"
 #include "dann_plan.h"
 
 #include <cub/device/device_radix_sort.cuh>
@@ -907,15 +908,11 @@ extern "C" int dann_search_batch_device(dann_index *ix, const float *d_queries, 
                                       d_out_tid, d_out_dist, nullptr, d_out_count, d_out_stats, st);
 } DANN_CATCH
 
-/* host-buffer batch with optional node ids (used by the scan operator too) */
-static int search_batch_host(dann_index *ix, const float *queries, const int16_t *labels,
-                             const int32_t *label_off, int B, int k, int L, int rescore, uint64_t *out_tid,
-                             float *out_dist, uint32_t *out_node, uint32_t *out_count,
-                             dann_query_stats *out_stats) {
-    int rc = check_live(ix);
-    if (rc) return rc;
-    if (B <= 0 || k <= 0 || !queries || !out_tid) return fail(DANN_ERR_INVALID_ARG, "dann_search_batch: bad argument");
-    std::lock_guard<std::mutex> lk(ix->mu);
+/* The device half of the host-buffer batch: stages B host queries (and label keys) on ix's device and runs the batch
+ * there.  Returns with the rows in ix->st_tid / st_dist / sc_node / st_count / st_stats and ix->stream drained.  The
+ * caller holds ix->mu. */
+static int search_batch_staged_locked(dann_index *ix, const float *queries, const int16_t *labels,
+                                      const int32_t *label_off, int B, int k, int L, int rescore) {
     cudaStream_t st = ix->stream;
     const IndexView &v = ix->v;
     const size_t nk = (size_t)B * k;
@@ -948,9 +945,23 @@ static int search_batch_host(dann_index *ix, const float *queries, const int16_t
         d_lab = ix->st_labels.as<int16_t>();
         d_off = ix->st_label_off.as<int32_t>();
     }
-    rc = search_batch_device_locked(ix, ix->st_queries.as<float>(), d_lab, d_off, B, k, L, rescore,
-                                    ix->st_tid.as<uint64_t>(), ix->st_dist.as<float>(), ix->sc_node.as<uint32_t>(),
-                                    ix->st_count.as<uint32_t>(), ix->st_stats.as<dann_query_stats>(), st);
+    return search_batch_device_locked(ix, ix->st_queries.as<float>(), d_lab, d_off, B, k, L, rescore,
+                                      ix->st_tid.as<uint64_t>(), ix->st_dist.as<float>(), ix->sc_node.as<uint32_t>(),
+                                      ix->st_count.as<uint32_t>(), ix->st_stats.as<dann_query_stats>(), st);
+}
+
+/* host-buffer batch with optional node ids (used by the scan operator too) */
+static int search_batch_host(dann_index *ix, const float *queries, const int16_t *labels,
+                             const int32_t *label_off, int B, int k, int L, int rescore, uint64_t *out_tid,
+                             float *out_dist, uint32_t *out_node, uint32_t *out_count,
+                             dann_query_stats *out_stats) {
+    int rc = check_live(ix);
+    if (rc) return rc;
+    if (B <= 0 || k <= 0 || !queries || !out_tid) return fail(DANN_ERR_INVALID_ARG, "dann_search_batch: bad argument");
+    std::lock_guard<std::mutex> lk(ix->mu);
+    cudaStream_t st = ix->stream;
+    const size_t nk = (size_t)B * k;
+    rc = search_batch_staged_locked(ix, queries, labels, label_off, B, k, L, rescore);
     if (rc) return rc;
     CK(cudaMemcpyAsync(out_tid, ix->st_tid.p, nk * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
     if (out_dist) CK(cudaMemcpyAsync(out_dist, ix->st_dist.p, nk * sizeof(float), cudaMemcpyDeviceToHost, st));
@@ -1699,6 +1710,16 @@ extern "C" void dann_scan_end(dann_scan *sc) {
 /* query coalescing for process-per-connection hosts (SURVEY.md §8f row 4)                */
 #include "dann_coalescer.h"
 #include "dann_group.h"
+
+/* ------------------------------------------------------------------------------------ */
+/* a table split into shards: every shard's batch, then one merge on the primary device   */
+/* the merge launch lives in this file, not in dann_shards.h: tests/simt/cu2cpp.py rewrites this file's launches only */
+static cudaError_t launch_shard_merge(const ShardMergeArgs &a, int sm_count, cudaStream_t st) {
+    const unsigned grid = (unsigned)std::max(1, std::min<int>((int)((a.B + DANN_MERGE_WARPS - 1) / DANN_MERGE_WARPS), sm_count));
+    dann_shard_merge_kernel<<<grid, DANN_MERGE_WARPS * 32, 0, st>>>(a);
+    return cudaGetLastError();
+}
+#include "dann_shards.h"
 
 /* ------------------------------------------------------------------------------------ */
 /* reading an index relation file (SURVEY.md §8f row 2): host only                       */

@@ -13,6 +13,7 @@ from __future__ import annotations
 
 import ctypes as C
 import os
+from types import SimpleNamespace
 from typing import Optional, Sequence
 
 import numpy as np
@@ -79,6 +80,7 @@ EXPORTS = [
     "dann_build_graph", "dann_index_download_nbrs", "dann_index_set_vectors", "dann_index_set_vectors_device",
     "dann_last_search_plan",
     "dann_group_create", "dann_group_size", "dann_group_replica", "dann_group_search_batch", "dann_group_free",
+    "dann_shards_create", "dann_shards_count", "dann_shards_index", "dann_shards_search_batch", "dann_shards_free",
     # relation-file reader (host only; mirror in pgreader.py)
     "dann_pg_relation_open", "dann_pg_relation_close", "dann_pg_relation_stat", "dann_pg_read_chain",
     "dann_pg_extract_sbq", "dann_pg_extract_plain", "dann_pg_snapshot_free", "dann_pg_heap_fetch_vectors",
@@ -136,6 +138,13 @@ def load_library(path: Optional[str] = None):
     lib.dann_group_search_batch.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp]
     lib.dann_group_free.argtypes = [vp]
     lib.dann_group_free.restype = None
+    lib.dann_shards_create.argtypes = [vp, C.c_int, vp, C.POINTER(vp)]
+    lib.dann_shards_count.argtypes = [vp]
+    lib.dann_shards_index.argtypes = [vp, C.c_int]
+    lib.dann_shards_index.restype = vp
+    lib.dann_shards_search_batch.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp]
+    lib.dann_shards_free.argtypes = [vp]
+    lib.dann_shards_free.restype = None
     lib.dann_coalescer_create.argtypes = [vp, C.c_int, C.c_int, C.POINTER(vp)]
     lib.dann_coalescer_search.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp]
     lib.dann_coalescer_gettuple.argtypes = [vp, vp, u32p, C.POINTER(C.c_uint16), u32p, C.POINTER(C.c_float)]
@@ -221,16 +230,28 @@ class DiskAnnIndex:
         else:
             _check(self._lib, self._lib.dann_index_load(C.byref(d), int(device), C.byref(h)))
         self._h = h
+        self._describe(s, device)
+
+    def _describe(self, s, device: int):
         self.device = int(device)
         self.n, self.dim, self.dim_index = s.n, s.dim, s.dim_index
         self.bits, self.words, self.R = s.bits, s.words, s.R
         self.distance_type = int(s.distance_type)
         self.has_labels = bool(s.has_labels)
 
+    @classmethod
+    def _view(cls, owner, handle, snapshot, device: int) -> "DiskAnnIndex":
+        """A non-owning DiskAnnIndex over an index handle that `owner` holds (and frees)."""
+        v = cls.__new__(cls)
+        v._lib, v._h, v._owner = owner._lib, C.c_void_p(handle), owner
+        v._describe(snapshot, device)
+        return v
+
     # -- lifetime -------------------------------------------------------------------
     def close(self):
         if getattr(self, "_h", None):
-            self._lib.dann_index_free(self._h)
+            if getattr(self, "_owner", None) is None:
+                self._lib.dann_index_free(self._h)
             self._h = None
 
     def __del__(self):
@@ -484,6 +505,79 @@ class IndexGroup:
     def close(self):
         if getattr(self, "_h", None):
             self._lib.dann_group_free(self._h)
+            self._h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.close()
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
+
+
+_GEOMETRY = ("n", "dim", "dim_index", "bits", "words", "R", "distance_type", "has_labels")
+
+
+class ShardedIndex:
+    """dann_shards: a table split into shards, one independent index per shard (its own graph, means and start nodes),
+    on one or several GPUs.  search_batch runs every shard on all queries and merges their rows on the device of shard
+    0: k times the head with the smallest (f32::total_cmp key of its distance, shard index) among the shards' lists."""
+
+    def __init__(self, snapshots: Sequence[Snapshot], devices: Optional[Sequence[int]] = None):
+        self._lib = load_library()
+        snaps = list(snapshots)
+        descs, keep = [], []
+        for s in snaps:
+            s.validate()
+            d, kp = _make_desc(s)
+            descs.append(d)
+            keep.append(kp)
+        arr = (C.POINTER(_SnapshotDesc) * max(len(descs), 1))(*[C.pointer(d) for d in descs])
+        devs = None if devices is None else np.ascontiguousarray(list(devices), dtype=np.int32)
+        h = C.c_void_p()
+        _check(self._lib, self._lib.dann_shards_create(C.cast(arr, C.c_void_p), len(descs), _np_ptr(devs), C.byref(h)))
+        self._h = h
+        self.dim = snaps[0].dim
+        self.count = int(self._lib.dann_shards_count(h))
+        self.devices = [int(x) for x in devs] if devs is not None else list(range(self.count))
+        # each shard's geometry for its view (not the arrays: the index has its own copy in HBM)
+        self._geom = [SimpleNamespace(**{f: getattr(s, f) for f in _GEOMETRY}) for s in snaps]
+        del keep
+
+    def shard(self, i: int) -> DiskAnnIndex:
+        """Shard i as a non-owning DiskAnnIndex (build_graph, set_vectors, set_vectors_device, last_batch_timing ...);
+        valid while this ShardedIndex is open."""
+        if not 0 <= i < self.count:
+            raise IndexError(f"shard {i} of {self.count}")
+        h = self._lib.dann_shards_index(self._h, int(i))
+        return DiskAnnIndex._view(self, h, self._geom[i], self.devices[i])
+
+    def search_batch(self, queries, labels=None, k: int = 10, search_list_size: int = QUERY_SEARCH_LIST_SIZE_DEFAULT,
+                     rescore: int = QUERY_RESCORE_DEFAULT) -> dict:
+        """Merged first k rows of B queries over every shard: dict(tid[B,k], dist[B,k], shard[B,k] i32 (-1 past count),
+        count[B], stats[nshards, B])."""
+        q = np.ascontiguousarray(queries, dtype=np.float32)
+        if q.ndim != 2 or q.shape[1] != self.dim:
+            raise ValueError(f"queries must be [B, {self.dim}]")
+        B = q.shape[0]
+        lab, off = DiskAnnIndex._labels_csr(labels, B)
+        out = dict(tid=np.empty((B, k), np.uint64), dist=np.empty((B, k), np.float32),
+                   shard=np.empty((B, k), np.int32), count=np.empty(B, np.uint32),
+                   stats=np.empty((self.count, B), STATS_DTYPE))
+        _check(self._lib, self._lib.dann_shards_search_batch(
+            self._h, _np_ptr(q), _np_ptr(lab) if lab is not None and lab.size else None, _np_ptr(off), B, int(k),
+            int(search_list_size), int(rescore), _np_ptr(out["tid"]), _np_ptr(out["dist"]), _np_ptr(out["shard"]),
+            _np_ptr(out["count"]), _np_ptr(out["stats"])))
+        return out
+
+    def close(self):
+        if getattr(self, "_h", None):
+            self._lib.dann_shards_free(self._h)
             self._h = None
 
     def __enter__(self):
