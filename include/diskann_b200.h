@@ -263,6 +263,40 @@ int dann_shards_search_batch(dann_shards *g, const float *queries, const int16_t
                              dann_query_stats *out_stats);
 void dann_shards_free(dann_shards *g);
 
+/* ---- streaming scan of a sharded table: amrescan, then amgettuple one row at a time over every shard -------------
+ * The scan operator of a sharded table, for a post-filter that is not a label key or a query without LIMIT: the batch's
+ * merge rule applied to unbounded streams.  A sharded scan holds one dann_scan per shard.
+ * - dann_shards_scan_rescan runs dann_scan_rescan on every shard with the same query, key, search_list_size and
+ *   rescore, and validates its arguments the way dann_scan_rescan does.  rescore == 0 is DANN_ERR_INVALID_ARG (rows
+ *   would carry no distance to merge on).  The shards of one device are prepared together and waited for with one
+ *   synchronisation per device.
+ * - dann_shards_scan_gettuple returns the head with the smallest (f32::total_cmp key of its distance, shard index)
+ *   among the shards whose scan has not ended, then advances that shard.  The first call after a rescan steps every
+ *   shard once to get its head: the shards of one device take that step together in one many-scan round (see
+ *   dann_scan_gettuple_many), all devices at the same time.  Every later call steps exactly one shard, the one whose
+ *   head the previous call returned, with an ordinary dann_scan_gettuple.  A shard whose step returns end of scan drops
+ *   out; the merged scan ends (0) when every shard has.  node_id is local to its shard, *shard says which shard (any
+ *   output pointer may be NULL).  Returns 1 (row), 0 (end of scan) or < 0.
+ * - Consequences: after any call, shard s has taken exactly as many amgettuple steps as this rule implies, and
+ *   dann_shards_scan_stats(out[s]) equals dann_scan_stats of a private scan of shard s after that many
+ *   dann_scan_gettuple calls (out has nshards entries).  For any k that dann_shards_search_batch accepts, the first k
+ *   rows of a sharded scan are exactly the batch's k rows: tid, distance bits and shard.
+ * - A shard's own failure fails the call as "shard i: ...".  A gettuple that fails, or a rescan that fails after its
+ *   arguments were checked, leaves the sharded scan unusable until the next successful rescan (DANN_ERR_STATE).
+ * - Threads: a sharded scan is single-threaded, like a dann_scan.  The handle serialises dann_shards_search_batch calls
+ *   only; every step of a scan or of a batch on a shard holds that shard's index lock (a first step or a rescan holds
+ *   the locks of several shards, taken in ascending shard order), so different sharded scans of one handle and
+ *   dann_shards_search_batch may be driven from different threads at once.  End every sharded scan before
+ *   dann_shards_free. */
+typedef struct dann_shards_scan dann_shards_scan;
+int dann_shards_scan_begin(dann_shards *g, dann_shards_scan **out);
+int dann_shards_scan_rescan(dann_shards_scan *sc, const float *query, const int16_t *labels, int nlabels,
+                            int search_list_size, int rescore);
+int dann_shards_scan_gettuple(dann_shards_scan *sc, uint32_t *block, uint16_t *offset, uint32_t *node_id, float *dist,
+                              int32_t *shard);
+int dann_shards_scan_stats(dann_shards_scan *sc, dann_query_stats *out /* [nshards] */);
+void dann_shards_scan_end(dann_shards_scan *sc);
+
 /* ---- reading an index RELATION FILE (SURVEY.md §8f row 2; pgvectorscale_b200/csrc/dann_pgreader.h) -------------------
  * Host-only, no GPU involved.  Replaces, for an external loader (the sidecar after a CHECKPOINT, an offline exporter):
  *   ReadablePage::read / get_type / get_item_unchecked   util/page.rs:254-290   dann_pg_relation_open / _info

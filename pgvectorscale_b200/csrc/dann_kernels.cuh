@@ -475,13 +475,14 @@ __global__ void __launch_bounds__(128) dann_scan_distance_kernel(IndexView ix, c
     scan_distance_step(ix, qs, &bar, q_full, stream, slen_p, overflow_p, skip, out);
 }
 
-/* One amgettuple step of many scans (dann_scan_gettuple_many): the arguments dann_scan_distance_kernel and
- * dann_scan_finish_kernel take, per scan. */
+/* One amgettuple step of many scans (dann_scan_gettuple_many, and the first step of a sharded scan): the arguments
+ * dann_scan_distance_kernel and dann_scan_finish_kernel take, per scan.  `view` picks the scan's index in the launch's
+ * table of IndexViews, so one launch can carry scans of several indexes on one device. */
 struct ScanDistanceDesc {
     const float *q_full;
     const uint32_t *stream, *slen_p, *overflow_p;
     float *out;
-    uint32_t skip, pad;
+    uint32_t skip, view;
 };
 struct ScanFinishDesc {
     ScanWindow *w;
@@ -491,16 +492,16 @@ struct ScanFinishDesc {
     const uint32_t *slen_p;     /* NULL: the scan did not search this step */
     const uint32_t *overflow_p; /* NULL: the scan did not search this step */
     const dann_query_stats *stats_p;
-    uint32_t rescore, skip, slen_fixed, pad;
+    uint32_t rescore, skip, slen_fixed, view;
 };
 
-/* CTA b: the exact distances of scan d[b], which searched with rescore > 0 */
-__global__ void __launch_bounds__(128) dann_scan_distance_many_kernel(IndexView ix, const ScanDistanceDesc *d) {
+/* CTA b: the exact distances of scan d[b], which searched with rescore > 0, on its index views[d[b].view] */
+__global__ void __launch_bounds__(128) dann_scan_distance_many_kernel(const IndexView *views, const ScanDistanceDesc *d) {
     DANN_DYN_SMEM(dann_smem);
     float *qs = reinterpret_cast<float *>(dann_smem);
     DANN_STATIC_SMEM uint64_t bar;
     const ScanDistanceDesc &e = d[blockIdx.x];
-    scan_distance_step(ix, qs, &bar, e.q_full, e.stream, e.slen_p, e.overflow_p, e.skip, e.out);
+    scan_distance_step(views[e.view], qs, &bar, e.q_full, e.stream, e.slen_p, e.overflow_p, e.skip, e.out);
 }
 
 /* The window step of one scan: next_with_resort's refill with the rows its search appended, then one pop; *out gathers
@@ -562,13 +563,14 @@ __global__ void dann_scan_finish_kernel(IndexView ix, ScanWindow *w, uint64_t *w
     scan_finish_step(ix, w, win, rescore, stream, dist, skip, slen_p, slen_fixed, overflow_p, stats_p, out);
 }
 
-/* thread i: the window step of scan d[i], its outcome into out[i] (one copy brings every scan's back) */
-__global__ void __launch_bounds__(128) dann_scan_finish_many_kernel(IndexView ix, const ScanFinishDesc *d, uint32_t n,
-                                                                    ScanStepOut *out) {
+/* thread i: the window step of scan d[i] on its index views[d[i].view], its outcome into out[i] (one copy brings every
+ * scan's back) */
+__global__ void __launch_bounds__(128) dann_scan_finish_many_kernel(const IndexView *views, const ScanFinishDesc *d,
+                                                                    uint32_t n, ScanStepOut *out) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const ScanFinishDesc f = d[i];
-    scan_finish_step(ix, f.w, f.win, f.rescore, f.stream, f.dist, f.skip, f.slen_p, f.slen_fixed, f.overflow_p, f.stats_p,
-                     out + i);
+    scan_finish_step(views[f.view], f.w, f.win, f.rescore, f.stream, f.dist, f.skip, f.slen_p, f.slen_fixed, f.overflow_p,
+                     f.stats_p, out + i);
 }
 

@@ -3,6 +3,8 @@
 // thread per distinct device, on WorkerLoop of dann_group.h), each worker copies its shards' rows into staging on the
 // primary device (shard 0's), and dann_shard_merge_kernel (dann_shards.cuh) merges them there.  No graph hop crosses a
 // device; only the merged k rows per query cross PCIe.
+// A sharded scan (dann_shards_scan) is one dann_scan per shard whose rows are merged on the host, one row per call; its
+// first step advances every device's shards in one dann_scan_gettuple_many round (scan_gettuple_many_locked).
 // Included at the end of diskann_b200.cu, after dann_group.h and launch_shard_merge().
 #pragma once
 
@@ -196,3 +198,198 @@ extern "C" int dann_shards_search_batch(dann_shards *g, const float *queries, co
 } DANN_CATCH
 
 #undef SK
+
+/* ---- streaming scan of a sharded table (include/diskann_b200.h, "streaming scan of a sharded table") ---- */
+
+/* f32::total_cmp as an unsigned key: total_ukey of dann_device.cuh, on the host */
+static uint32_t host_total_ukey(float f) {
+    uint32_t b;
+    memcpy(&b, &f, sizeof b);
+    return (b >> 31) ? ~b : (b | 0x80000000u);
+}
+
+struct dann_shards_scan {
+    dann_shards *g = nullptr;
+    std::vector<dann_scan *> sc; /* shard s's own scan */
+    struct Head {
+        uint32_t block = 0, node = 0;
+        uint16_t offset = 0;
+        float dist = 0.0f;
+        bool live = false; /* a row of the shard is waiting to be merged */
+    };
+    std::vector<Head> head;
+    int step_next = -1;  /* the shard whose head the last call returned: the next call steps it */
+    bool first = true;   /* no shard has stepped since the rescan */
+    bool active = false; /* rescanned, and no call has failed since */
+};
+
+extern "C" void dann_shards_scan_end(dann_shards_scan *ss) {
+    if (!ss) return;
+    for (dann_scan *sc : ss->sc) dann_scan_end(sc);
+    delete ss;
+}
+
+extern "C" int dann_shards_scan_begin(dann_shards *g, dann_shards_scan **out) try {
+    if (!g || !out) return fail(DANN_ERR_INVALID_ARG, "dann_shards_scan_begin: NULL argument");
+    *out = nullptr;
+    dann_shards_scan *ss = new dann_shards_scan();
+    ss->g = g;
+    ss->head.resize(g->ix.size());
+    ss->sc.reserve(g->ix.size());
+    for (dann_index *ix : g->ix) {
+        dann_scan *sc = nullptr;
+        const int rc = dann_scan_begin(ix, &sc);
+        if (rc) {
+            dann_shards_scan_end(ss);
+            return rc;
+        }
+        ss->sc.push_back(sc);
+    }
+    *out = ss;
+    return DANN_OK;
+} DANN_CATCH
+
+/* the failure of shard s's own call, with g_err as its message */
+static int shard_failed(int s, int rc) {
+    const std::string keep = g_err;
+    return fail(rc, "shard %d: %s", s, keep.c_str());
+}
+
+extern "C" int dann_shards_scan_rescan(dann_shards_scan *ss, const float *query, const int16_t *labels, int nlabels,
+                                       int search_list_size, int rescore) try {
+    if (!ss) return fail(DANN_ERR_INVALID_ARG, "dann_shards_scan_rescan: NULL scan");
+    int rc = scan_rescan_check(labels, nlabels, search_list_size, rescore);
+    if (rc) return rc;
+    if (rescore == 0) return fail(DANN_ERR_INVALID_ARG, "dann_shards_scan_rescan: rescore 0 leaves the rows without a distance to merge on");
+    dann_shards *g = ss->g;
+    ss->active = false;
+    ss->first = true;
+    ss->step_next = -1;
+    for (dann_shards_scan::Head &h : ss->head) h = dann_shards_scan::Head{};
+    std::vector<std::unique_lock<std::mutex>> locks;
+    locks.reserve(g->ix.size());
+    for (dann_index *ix : g->ix) locks.emplace_back(ix->mu); /* ascending shard order */
+    /* each device's shards are enqueued on the stream of its first shard, then every device is waited for once */
+    for (const std::vector<int> &dev : g->of_dev) {
+        cudaStream_t st = g->ix[(size_t)dev[0]]->stream;
+        for (int s : dev) {
+            rc = check_live(g->ix[(size_t)s]);
+            if (!rc) rc = scan_rescan_enqueue(ss->sc[(size_t)s], query, labels, nlabels, search_list_size, rescore, st);
+            if (rc) return shard_failed(s, rc);
+        }
+    }
+    std::vector<dann_scan *> scans;
+    for (const std::vector<int> &dev : g->of_dev) {
+        dann_index *lead = g->ix[(size_t)dev[0]];
+        scans.clear();
+        for (int s : dev) scans.push_back(ss->sc[(size_t)s]);
+        rc = check_live(lead);
+        if (!rc) rc = scan_rescan_wait(lead, lead->stream, scans.data(), scans.size());
+        if (rc) return shard_failed(dev[0], rc);
+    }
+    ss->active = true;
+    return DANN_OK;
+} DANN_CATCH
+
+/* The first step of the scans of device w's shards: one dann_scan_gettuple_many round (or a few, when a scan regrows)
+ * that carries all of them, on the stream of the device's first shard, under the shards' mutexes in ascending order. */
+static int shards_scan_first_step_on(dann_shards_scan *ss, size_t w) {
+    dann_shards *g = ss->g;
+    const std::vector<int> &dev = g->of_dev[w];
+    const size_t n = dev.size();
+    std::vector<std::unique_lock<std::mutex>> locks;
+    std::vector<dann_scan *> scans;
+    locks.reserve(n);
+    for (int s : dev) {
+        dann_index *ix = g->ix[(size_t)s];
+        const int rc = check_live(ix);
+        if (rc) return shard_failed(s, rc);
+        locks.emplace_back(ix->mu);
+        scans.push_back(ss->sc[(size_t)s]);
+    }
+    std::vector<int32_t> out_rc(n, 0);
+    std::vector<uint32_t> block(n), node(n);
+    std::vector<uint16_t> offset(n);
+    std::vector<float> dist(n);
+    std::vector<std::string> msgs;
+    int rc = scan_gettuple_many_locked(g->ix[(size_t)dev[0]], scans.data(), (int)n, out_rc.data(), block.data(),
+                                       offset.data(), node.data(), dist.data(), &msgs);
+    if (rc) return shard_failed(dev[0], rc);
+    for (size_t j = 0; j < n; j++) {
+        if (out_rc[j] < 0) return fail(out_rc[j], "shard %d: %s", dev[j], msgs[j].c_str());
+        ss->head[(size_t)dev[j]] = dann_shards_scan::Head{block[j], node[j], offset[j], dist[j], out_rc[j] == 1};
+    }
+    return DANN_OK;
+}
+
+/* The first step of every shard: one round per device, the devices at the same time (the first on this thread). */
+static int shards_scan_first_step(dann_shards_scan *ss) {
+    const size_t D = ss->g->of_dev.size();
+    std::vector<int> rc(D, DANN_OK);
+    std::vector<std::string> err(D);
+    auto run = [&](size_t w) {
+        try {
+            rc[w] = shards_scan_first_step_on(ss, w);
+            if (rc[w]) err[w] = g_err; /* thread-local message of this thread */
+        } catch (const std::bad_alloc &) {
+            rc[w] = DANN_ERR_OOM;
+        } catch (...) {
+            rc[w] = DANN_ERR_STATE;
+        }
+    };
+    std::vector<std::thread> th;
+    th.reserve(D);
+    for (size_t w = 1; w < D; w++) th.emplace_back(run, w);
+    run(0);
+    for (std::thread &t : th) t.join();
+    for (size_t w = 0; w < D; w++)
+        if (rc[w]) return fail(rc[w], "%s", err[w].empty() ? "host failure in a first step" : err[w].c_str());
+    return DANN_OK;
+}
+
+extern "C" int dann_shards_scan_gettuple(dann_shards_scan *ss, uint32_t *block, uint16_t *offset, uint32_t *node_id,
+                                         float *dist, int32_t *shard) try {
+    if (!ss) return fail(DANN_ERR_INVALID_ARG, "dann_shards_scan_gettuple: NULL scan");
+    if (!ss->active) return fail(DANN_ERR_STATE, "dann_shards_scan_gettuple before dann_shards_scan_rescan, or after a failed call");
+    ss->active = false; /* until this call has succeeded */
+    if (ss->first) {
+        const int rc = shards_scan_first_step(ss);
+        if (rc) return rc;
+        ss->first = false;
+    } else if (ss->step_next >= 0) {
+        const int s = ss->step_next;
+        dann_shards_scan::Head &h = ss->head[(size_t)s];
+        const int rc = dann_scan_gettuple(ss->sc[(size_t)s], &h.block, &h.offset, &h.node, &h.dist);
+        if (rc < 0) return shard_failed(s, rc);
+        h.live = rc == 1;
+    }
+    ss->active = true;
+    ss->step_next = -1;
+    int best = -1;
+    uint32_t best_key = 0;
+    for (size_t s = 0; s < ss->head.size(); s++) {
+        const dann_shards_scan::Head &h = ss->head[s];
+        if (!h.live) continue;
+        const uint32_t key = host_total_ukey(h.dist);
+        if (best < 0 || key < best_key) { /* ties: the lower shard */
+            best = (int)s;
+            best_key = key;
+        }
+    }
+    if (best < 0) return 0;
+    dann_shards_scan::Head &h = ss->head[(size_t)best];
+    if (block) *block = h.block;
+    if (offset) *offset = h.offset;
+    if (node_id) *node_id = h.node;
+    if (dist) *dist = h.dist;
+    if (shard) *shard = best;
+    h.live = false;
+    ss->step_next = best;
+    return 1;
+} DANN_CATCH
+
+extern "C" int dann_shards_scan_stats(dann_shards_scan *ss, dann_query_stats *out) try {
+    if (!ss || !out) return fail(DANN_ERR_INVALID_ARG, "dann_shards_scan_stats: NULL argument");
+    for (size_t s = 0; s < ss->sc.size(); s++) out[s] = ss->sc[s]->stats;
+    return DANN_OK;
+} DANN_CATCH

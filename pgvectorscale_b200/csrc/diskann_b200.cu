@@ -1249,10 +1249,9 @@ static void scan_release(dann_scan *sc) {
     for (DevBuf *b : bufs) b->release();
 }
 
-/* (re)allocate the scan's private workspace for the current plan and reset the search state */
-static int scan_reset_search(dann_scan *sc) {
+/* (re)allocate the scan's private workspace for the current plan and reset the search state, enqueued on `st` */
+static int scan_reset_search(dann_scan *sc, cudaStream_t st) {
     dann_index *ix = sc->ix;
-    cudaStream_t st = ix->stream;
     SearchPlan &p = sc->plan;
     int rc = make_plan(ix, 1, (uint32_t)sc->L, (uint32_t)sc->rescore + 64u, sc->grow, sc->nlabels >= 0, &p, true);
     if (rc) return rc;
@@ -1272,23 +1271,27 @@ static int scan_reset_search(dann_scan *sc) {
     return DANN_OK;
 }
 
-extern "C" int dann_scan_rescan(dann_scan *sc, const float *query, const int16_t *labels, int nlabels,
-                                int search_list_size, int rescore) try {
-    if (!sc) return fail(DANN_ERR_INVALID_ARG, "dann_scan_rescan: NULL scan");
+/* amrescan's checks of its arguments that do not depend on the index */
+static int scan_rescan_check(const int16_t *labels, int nlabels, int search_list_size, int rescore) {
     if (search_list_size < 1 || search_list_size > 10000) return fail(DANN_ERR_INVALID_ARG, "search_list_size %d outside 1..10000", search_list_size);
     if (rescore < 0 || rescore > 1000) return fail(DANN_ERR_INVALID_ARG, "rescore %d outside 0..1000", rescore);
     if (nlabels > 0 && !labels) return fail(DANN_ERR_INVALID_ARG, "labels is NULL but nlabels > 0");
+    return DANN_OK;
+}
+
+/* The enqueue half of amrescan: the scan's new query, key and parameters, and its vector preparation and search reset
+ * enqueued on `st`, a stream of the index's device.  The caller has checked the arguments (scan_rescan_check), made the
+ * device current and holds sc->ix->mu; the scan may step once `st` has been synchronised (scan_rescan_wait).  Several
+ * scans may be enqueued on one stream and waited for with one synchronisation. */
+static int scan_rescan_enqueue(dann_scan *sc, const float *query, const int16_t *labels, int nlabels,
+                               int search_list_size, int rescore, cudaStream_t st) {
     dann_index *ix = sc->ix;
-    int rc = check_live(ix);
-    if (rc) return rc;
-    std::lock_guard<std::mutex> lk(ix->mu);
     const IndexView &v = ix->v;
     if (ix->plain) {
         if (query && nlabels >= 0) return fail(DANN_ERR_INVALID_ARG, "plain storage does not support label filters (plain/storage.rs:260)");
         if (v.dim == v.dim_index) rescore = 0; /* scan.rs:392-403: next() instead of next_with_resort */
     }
     if (rescore > 0 && v.n && !v.vectors) return fail(DANN_ERR_STATE, "index has no heap vectors yet: rescore must be 0");
-    cudaStream_t st = ix->stream;
     const uint32_t dim = v.dim;
     if (query) sc->query.assign(query, query + dim);
     else sc->query.assign(dim, 0.0f); /* NULL order-by argument: zero vector, no labels (labels/mod.rs:214-216) */
@@ -1321,14 +1324,32 @@ extern "C" int dann_scan_rescan(dann_scan *sc, const float *query, const int16_t
     }
     CK(cudaMemsetAsync(sc->d_winst.p, 0, sizeof(ScanWindow), st));
     if (ix->plain) CK(sc->d_qindex.reserve((size_t)v.dim_index * 4));
-    rc = launch_prepare(ix, sc->d_query.as<float>(), 1, sc->d_qfull.as<float>(), sc->d_qcodes.as<uint64_t>(),
-                        sc->d_qindex.as<float>(), st);
+    int rc = launch_prepare(ix, sc->d_query.as<float>(), 1, sc->d_qfull.as<float>(), sc->d_qcodes.as<uint64_t>(),
+                            sc->d_qindex.as<float>(), st);
     if (rc) return rc;
-    rc = scan_reset_search(sc);
-    if (rc) return rc;
+    return scan_reset_search(sc, st);
+}
+
+/* The wait half of amrescan: one synchronisation of `st`, on which the n scans of `ix`'s device were enqueued; then they
+ * may step. */
+static int scan_rescan_wait(dann_index *ix, cudaStream_t st, dann_scan *const *scans, size_t n) {
     CK(cudaStreamSynchronize(st));
-    sc->active = true;
+    for (size_t i = 0; i < n; i++) scans[i]->active = true;
     return DANN_OK;
+}
+
+extern "C" int dann_scan_rescan(dann_scan *sc, const float *query, const int16_t *labels, int nlabels,
+                                int search_list_size, int rescore) try {
+    if (!sc) return fail(DANN_ERR_INVALID_ARG, "dann_scan_rescan: NULL scan");
+    int rc = scan_rescan_check(labels, nlabels, search_list_size, rescore);
+    if (rc) return rc;
+    dann_index *ix = sc->ix;
+    rc = check_live(ix);
+    if (rc) return rc;
+    std::lock_guard<std::mutex> lk(ix->mu);
+    rc = scan_rescan_enqueue(sc, query, labels, nlabels, search_list_size, rescore, ix->stream);
+    if (rc) return rc;
+    return scan_rescan_wait(ix, ix->stream, &sc, 1);
 } DANN_CATCH
 
 /* The launch arguments of the scan's resumable search for rows [0, want) of this step: its plan, its private workspace
@@ -1400,7 +1421,7 @@ static int scan_distance_desc(dann_scan *sc, uint32_t want, uint32_t skip, ScanD
     dann_index *ix = sc->ix;
     CK(sc->d_dist.reserve((size_t)want * 4));
     *d = ScanDistanceDesc{sc->d_qfull.as<float>(), sc->d_stream.as<uint32_t>(), sc->d_slen.as<uint32_t>(),
-                          sc->d_ctl.as<uint32_t>() + 1, sc->d_dist.as<float>(), skip, 0u};
+                          sc->d_ctl.as<uint32_t>() + 1, sc->d_dist.as<float>(), skip, 0u /* view */};
     return DANN_OK;
 }
 
@@ -1417,15 +1438,16 @@ static ScanFinishDesc scan_finish_desc(dann_scan *sc, bool searching, uint32_t s
     f.rescore = (uint32_t)sc->rescore;
     f.skip = skip;
     f.slen_fixed = skip;
-    f.pad = 0;
+    f.view = 0;
     return f;
 }
 
-/* the scan outgrew its workspace: rebuild it twice as large; the next search replays the stream up to sc->streamed */
-static int scan_regrow(dann_scan *sc, int attempt) {
+/* the scan outgrew its workspace: rebuild it twice as large (its reset enqueued on `st`, the stream its next search
+ * runs on); the next search replays the stream up to sc->streamed */
+static int scan_regrow(dann_scan *sc, int attempt, cudaStream_t st) {
     if (attempt >= 8) return fail(DANN_ERR_CAPACITY, "scan workspace still too small after %d growth steps", attempt);
     sc->grow *= 2;
-    return scan_reset_search(sc);
+    return scan_reset_search(sc, st);
 }
 
 /* The host side of a step that did not overflow: the stream position, end of stream and counters of the scan, then its
@@ -1493,33 +1515,38 @@ extern "C" int dann_scan_gettuple(dann_scan *sc, uint32_t *block, uint16_t *offs
         CK(cudaMemcpyAsync(&o, sc->d_step.p, sizeof o, cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
         if (!o.overflow) break;
-        rc = scan_regrow(sc, attempt);
+        rc = scan_regrow(sc, attempt, st);
         if (rc) return rc;
         skip = sc->streamed;
     }
     return scan_after_step(sc, o, searching, skip + need, skip, block, offset, node_id, dist);
 } DANN_CATCH
 
-/* The device part of one dann_scan_gettuple_many round: one upload of [SearchArgs x args][ScanDistanceDesc x ddesc]
- * [ScanFinishDesc x fdesc], one dann_scan_search_many_kernel launch per run of equal fns[] (args is grouped by
- * instantiation), one dann_scan_distance_many_kernel launch when ddesc is not empty, one dann_scan_finish_many_kernel
- * launch, one download of the fdesc.size() outcomes into outs and one synchronisation. */
-static int scan_many_round(dann_index *ix, const std::vector<scan_many_fn> &fns, const std::vector<SearchArgs> &args,
-                           const std::vector<ScanDistanceDesc> &ddesc, const std::vector<ScanFinishDesc> &fdesc,
-                           std::vector<unsigned char> &blob, std::vector<ScanStepOut> &outs) {
-    const IndexView &v = ix->v;
+/* The device part of one dann_scan_gettuple_many round: one upload of [IndexView x views][SearchArgs x args]
+ * [ScanDistanceDesc x ddesc][ScanFinishDesc x fdesc], one dann_scan_search_many_kernel launch per run of equal fns[]
+ * (args is grouped by instantiation), one dann_scan_distance_many_kernel launch when ddesc is not empty, one
+ * dann_scan_finish_many_kernel launch, one download of the fdesc.size() outcomes into outs and one synchronisation.
+ * The descriptors' `view` fields index views[]: the indexes of the round's scans, all on the device of `ix`, whose
+ * stream, sc_many buffer and launch counter the round uses. */
+static int scan_many_round(dann_index *ix, const std::vector<IndexView> &views, const std::vector<scan_many_fn> &fns,
+                           const std::vector<SearchArgs> &args, const std::vector<ScanDistanceDesc> &ddesc,
+                           const std::vector<ScanFinishDesc> &fdesc, std::vector<unsigned char> &blob,
+                           std::vector<ScanStepOut> &outs) {
     cudaStream_t st = ix->stream;
     const size_t m = fdesc.size();
     auto align16 = [](size_t b) { return (b + 15) & ~(size_t)15; };
-    const size_t o_dist = align16(args.size() * sizeof(SearchArgs));
+    const size_t o_args = align16(views.size() * sizeof(IndexView));
+    const size_t o_dist = o_args + align16(args.size() * sizeof(SearchArgs));
     const size_t o_fin = o_dist + align16(ddesc.size() * sizeof(ScanDistanceDesc));
     const size_t o_out = o_fin + align16(m * sizeof(ScanFinishDesc));
     blob.assign(o_out, 0);
-    if (!args.empty()) memcpy(blob.data(), args.data(), args.size() * sizeof(SearchArgs));
+    memcpy(blob.data(), views.data(), views.size() * sizeof(IndexView));
+    if (!args.empty()) memcpy(blob.data() + o_args, args.data(), args.size() * sizeof(SearchArgs));
     if (!ddesc.empty()) memcpy(blob.data() + o_dist, ddesc.data(), ddesc.size() * sizeof(ScanDistanceDesc));
     memcpy(blob.data() + o_fin, fdesc.data(), m * sizeof(ScanFinishDesc));
     CK(ix->sc_many.reserve(o_out + m * sizeof(ScanStepOut)));
     unsigned char *dev = ix->sc_many.as<unsigned char>();
+    const IndexView *d_views = reinterpret_cast<const IndexView *>(dev);
     CK(cudaMemcpyAsync(dev, blob.data(), o_out, cudaMemcpyHostToDevice, st));
     for (size_t g = 0; g < args.size();) {
         size_t e = g;
@@ -1528,21 +1555,22 @@ static int scan_many_round(dann_index *ix, const std::vector<scan_many_fn> &fns,
         const scan_many_fn fn = fns[g];
         const size_t smem = (size_t)per_warp + DANN_SMEM_SLACK;
         CK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        fn<<<(unsigned)(e - g), 32, smem, st>>>(reinterpret_cast<const SearchArgs *>(dev) + g, (uint32_t)(e - g));
+        fn<<<(unsigned)(e - g), 32, smem, st>>>(reinterpret_cast<const SearchArgs *>(dev + o_args) + g, (uint32_t)(e - g));
         ix->launches++;
         CK(cudaGetLastError());
         g = e;
     }
     if (!ddesc.empty()) {
-        const size_t smem = scan_distance_smem(v);
+        size_t smem = 0;
+        for (const IndexView &v : views) smem = std::max(smem, scan_distance_smem(v));
         CK(allow_dynamic_smem(dann_scan_distance_many_kernel, smem));
         dann_scan_distance_many_kernel<<<(unsigned)ddesc.size(), 128, smem, st>>>(
-            v, reinterpret_cast<const ScanDistanceDesc *>(dev + o_dist));
+            d_views, reinterpret_cast<const ScanDistanceDesc *>(dev + o_dist));
         ix->launches++;
         CK(cudaGetLastError());
     }
     dann_scan_finish_many_kernel<<<(unsigned)((m + 127) / 128), 128, 0, st>>>(
-        v, reinterpret_cast<const ScanFinishDesc *>(dev + o_fin), (uint32_t)m, reinterpret_cast<ScanStepOut *>(dev + o_out));
+        d_views, reinterpret_cast<const ScanFinishDesc *>(dev + o_fin), (uint32_t)m, reinterpret_cast<ScanStepOut *>(dev + o_out));
     ix->launches++;
     CK(cudaGetLastError());
     outs.resize(m);
@@ -1551,12 +1579,138 @@ static int scan_many_round(dann_index *ix, const std::vector<scan_many_fn> &fns,
     return DANN_OK;
 }
 
-/* One amgettuple of each of n scans of one index, in rounds (scan_many_round).  The first round takes every scan; a
- * scan whose search overflowed regrows alone and replays in the next round, with the others done.
+/* One amgettuple of each of n scans, in rounds (scan_many_round) on the stream of `lead`.  The scans may belong to
+ * several indexes on the device of `lead`; the caller has checked the arguments, made the device current and holds
+ * the mutex of every index involved.  The first round takes every scan; a scan whose search overflowed regrows alone
+ * and replays in the next round, with the others done.
  * What fails for one scan (its workspace cannot grow, or its buffers cannot be allocated) goes to that scan's out_rc
  * and, when msgs != NULL, its message to (*msgs)[i]; the other scans go on.  A failure of a round as a whole fails the
  * call only while no scan has taken its step yet; after that it goes to the out_rc of every scan of the round, so that
  * no scan's row is lost. */
+static int scan_gettuple_many_locked(dann_index *lead, dann_scan *const *scans, int n, int32_t *out_rc, uint32_t *block,
+                                     uint16_t *offset, uint32_t *node_id, float *dist, std::vector<std::string> *msgs) {
+    int rc = DANN_OK;
+    struct Step {
+        dann_scan *sc;
+        int i;            /* position in the caller's arrays */
+        uint32_t need, skip;
+        bool searching;
+        int attempt;
+        scan_many_fn fn;  /* its search instantiation */
+        uint32_t view;    /* its index in views[] */
+    };
+    /* everything the rounds use is allocated here, before any scan moves: a host allocation failure later would fail
+     * the call after some scans have taken their step */
+    std::vector<Step> steps((size_t)n);
+    std::vector<Step *> round((size_t)n), searchers, live, next;
+    std::vector<const dann_index *> indexes;
+    std::vector<IndexView> views;
+    std::vector<scan_many_fn> fns;
+    std::vector<SearchArgs> args;
+    std::vector<ScanDistanceDesc> ddesc;
+    std::vector<ScanFinishDesc> fdesc;
+    std::vector<unsigned char> blob;
+    std::vector<ScanStepOut> outs;
+    searchers.reserve(n);
+    live.reserve(n);
+    next.reserve(n);
+    fns.reserve(n);
+    args.reserve(n);
+    ddesc.reserve(n);
+    fdesc.reserve(n);
+    outs.reserve(n);
+    if (msgs) msgs->assign((size_t)n, std::string());
+    for (int i = 0; i < n; i++) {
+        dann_scan *sc = scans[i];
+        const size_t view = (size_t)(std::find(indexes.begin(), indexes.end(), sc->ix) - indexes.begin());
+        if (view == indexes.size()) {
+            indexes.push_back(sc->ix);
+            views.push_back(sc->ix->v);
+        }
+        const uint32_t need = scan_step_need(sc);
+        steps[i] = Step{sc, i, need, 0u, need && !sc->exhausted, 0, nullptr, (uint32_t)view};
+        round[i] = &steps[i];
+    }
+    blob.reserve(views.size() * sizeof(IndexView) +
+                 (size_t)n * (sizeof(SearchArgs) + sizeof(ScanDistanceDesc) + sizeof(ScanFinishDesc)) + 64);
+    bool moved = false; /* some scan has taken its step */
+    auto scan_failed = [&](const Step *s, int code) {
+        out_rc[s->i] = code;
+        if (msgs) {
+            try {
+                (*msgs)[s->i] = g_err;
+            } catch (...) { /* no memory for the message: the code still goes back */
+            }
+        }
+    };
+    while (!round.empty()) {
+        /* the searching scans, grouped by instantiation: one launch per group */
+        searchers.clear();
+        for (Step *s : round)
+            if (s->searching) {
+                s->fn = pick_scan_many(s->sc->plan.entry, s->sc->ix->NCH, s->sc->ix->plain);
+                searchers.push_back(s);
+            }
+        std::stable_sort(searchers.begin(), searchers.end(),
+                         [](const Step *a, const Step *b) { return (uintptr_t)a->fn < (uintptr_t)b->fn; });
+        fns.clear();
+        args.clear();
+        ddesc.clear();
+        for (Step *s : searchers) {
+            const uint32_t want = s->skip + s->need;
+            SearchArgs a;
+            ScanDistanceDesc d{};
+            rc = scan_search_args(s->sc, want, &a);
+            if (!rc && s->sc->rescore > 0) rc = scan_distance_desc(s->sc, want, s->skip, &d);
+            if (rc) { /* this scan's buffers: it leaves the round */
+                scan_failed(s, rc);
+                s->fn = nullptr;
+                continue;
+            }
+            d.view = s->view;
+            fns.push_back(s->fn);
+            args.push_back(a);
+            if (s->sc->rescore > 0) ddesc.push_back(d);
+        }
+        live.clear();
+        fdesc.clear();
+        for (Step *s : round)
+            if (!s->searching || s->fn) {
+                live.push_back(s);
+                fdesc.push_back(scan_finish_desc(s->sc, s->searching, s->skip));
+                fdesc.back().view = s->view;
+            }
+        if (live.empty()) break;
+        rc = scan_many_round(lead, views, fns, args, ddesc, fdesc, blob, outs);
+        if (rc) {
+            if (!moved) return rc;
+            for (Step *s : live) scan_failed(s, rc);
+            break;
+        }
+        next.clear();
+        for (size_t j = 0; j < live.size(); j++) {
+            Step *s = live[j];
+            const int i = s->i;
+            if (!outs[j].overflow) {
+                out_rc[i] = scan_after_step(s->sc, outs[j], s->searching, s->skip + s->need, s->skip, block ? block + i : nullptr,
+                                            offset ? offset + i : nullptr, node_id ? node_id + i : nullptr, dist ? dist + i : nullptr);
+                moved = true;
+                continue;
+            }
+            rc = scan_regrow(s->sc, s->attempt++, lead->stream);
+            if (rc) { /* capacity, memory, or a CUDA error that has poisoned the handle: this scan alone */
+                scan_failed(s, rc);
+                continue;
+            }
+            s->skip = s->sc->streamed;
+            next.push_back(s);
+        }
+        round.swap(next);
+    }
+    return DANN_OK;
+}
+
+/* dann_scan_gettuple_many: n scans of one index */
 static int scan_gettuple_many(dann_scan *const *scans, int n, int32_t *out_rc, uint32_t *block, uint16_t *offset,
                               uint32_t *node_id, float *dist, std::vector<std::string> *msgs) {
     if (!scans || !out_rc) return fail(DANN_ERR_INVALID_ARG, "dann_scan_gettuple_many: NULL argument");
@@ -1577,114 +1731,7 @@ static int scan_gettuple_many(dann_scan *const *scans, int n, int32_t *out_rc, u
     int rc = check_live(ix);
     if (rc) return rc;
     std::lock_guard<std::mutex> lk(ix->mu);
-
-    struct Step {
-        dann_scan *sc;
-        int i;            /* position in the caller's arrays */
-        uint32_t need, skip;
-        bool searching;
-        int attempt;
-        scan_many_fn fn;  /* its search instantiation */
-    };
-    /* everything the rounds use is allocated here, before any scan moves: a host allocation failure later would fail
-     * the call after some scans have taken their step */
-    std::vector<Step> steps((size_t)n);
-    std::vector<Step *> round((size_t)n), searchers, live, next;
-    std::vector<scan_many_fn> fns;
-    std::vector<SearchArgs> args;
-    std::vector<ScanDistanceDesc> ddesc;
-    std::vector<ScanFinishDesc> fdesc;
-    std::vector<unsigned char> blob;
-    std::vector<ScanStepOut> outs;
-    searchers.reserve(n);
-    live.reserve(n);
-    next.reserve(n);
-    fns.reserve(n);
-    args.reserve(n);
-    ddesc.reserve(n);
-    fdesc.reserve(n);
-    outs.reserve(n);
-    blob.reserve((size_t)n * (sizeof(SearchArgs) + sizeof(ScanDistanceDesc) + sizeof(ScanFinishDesc)) + 64);
-    if (msgs) msgs->assign((size_t)n, std::string());
-    for (int i = 0; i < n; i++) {
-        dann_scan *sc = scans[i];
-        const uint32_t need = scan_step_need(sc);
-        steps[i] = Step{sc, i, need, 0u, need && !sc->exhausted, 0, nullptr};
-        round[i] = &steps[i];
-    }
-    bool moved = false; /* some scan has taken its step */
-    auto scan_failed = [&](const Step *s, int code) {
-        out_rc[s->i] = code;
-        if (msgs) {
-            try {
-                (*msgs)[s->i] = g_err;
-            } catch (...) { /* no memory for the message: the code still goes back */
-            }
-        }
-    };
-    while (!round.empty()) {
-        /* the searching scans, grouped by instantiation: one launch per group */
-        searchers.clear();
-        for (Step *s : round)
-            if (s->searching) {
-                s->fn = pick_scan_many(s->sc->plan.entry, ix->NCH, ix->plain);
-                searchers.push_back(s);
-            }
-        std::stable_sort(searchers.begin(), searchers.end(),
-                         [](const Step *a, const Step *b) { return (uintptr_t)a->fn < (uintptr_t)b->fn; });
-        fns.clear();
-        args.clear();
-        ddesc.clear();
-        for (Step *s : searchers) {
-            const uint32_t want = s->skip + s->need;
-            SearchArgs a;
-            ScanDistanceDesc d{};
-            rc = scan_search_args(s->sc, want, &a);
-            if (!rc && s->sc->rescore > 0) rc = scan_distance_desc(s->sc, want, s->skip, &d);
-            if (rc) { /* this scan's buffers: it leaves the round */
-                scan_failed(s, rc);
-                s->fn = nullptr;
-                continue;
-            }
-            fns.push_back(s->fn);
-            args.push_back(a);
-            if (s->sc->rescore > 0) ddesc.push_back(d);
-        }
-        live.clear();
-        fdesc.clear();
-        for (Step *s : round)
-            if (!s->searching || s->fn) {
-                live.push_back(s);
-                fdesc.push_back(scan_finish_desc(s->sc, s->searching, s->skip));
-            }
-        if (live.empty()) break;
-        rc = scan_many_round(ix, fns, args, ddesc, fdesc, blob, outs);
-        if (rc) {
-            if (!moved) return rc;
-            for (Step *s : live) scan_failed(s, rc);
-            break;
-        }
-        next.clear();
-        for (size_t j = 0; j < live.size(); j++) {
-            Step *s = live[j];
-            const int i = s->i;
-            if (!outs[j].overflow) {
-                out_rc[i] = scan_after_step(s->sc, outs[j], s->searching, s->skip + s->need, s->skip, block ? block + i : nullptr,
-                                            offset ? offset + i : nullptr, node_id ? node_id + i : nullptr, dist ? dist + i : nullptr);
-                moved = true;
-                continue;
-            }
-            rc = scan_regrow(s->sc, s->attempt++);
-            if (rc) { /* capacity, memory, or a CUDA error that has poisoned the handle: this scan alone */
-                scan_failed(s, rc);
-                continue;
-            }
-            s->skip = s->sc->streamed;
-            next.push_back(s);
-        }
-        round.swap(next);
-    }
-    return DANN_OK;
+    return scan_gettuple_many_locked(ix, scans, n, out_rc, block, offset, node_id, dist, msgs);
 }
 
 extern "C" int dann_scan_gettuple_many(dann_scan *const *scans, int n, int32_t *out_rc, uint32_t *block, uint16_t *offset,

@@ -81,6 +81,8 @@ EXPORTS = [
     "dann_last_search_plan",
     "dann_group_create", "dann_group_size", "dann_group_replica", "dann_group_search_batch", "dann_group_free",
     "dann_shards_create", "dann_shards_count", "dann_shards_index", "dann_shards_search_batch", "dann_shards_free",
+    "dann_shards_scan_begin", "dann_shards_scan_rescan", "dann_shards_scan_gettuple", "dann_shards_scan_stats",
+    "dann_shards_scan_end",
     # relation-file reader (host only; mirror in pgreader.py)
     "dann_pg_relation_open", "dann_pg_relation_close", "dann_pg_relation_stat", "dann_pg_read_chain",
     "dann_pg_extract_sbq", "dann_pg_extract_plain", "dann_pg_snapshot_free", "dann_pg_heap_fetch_vectors",
@@ -145,6 +147,13 @@ def load_library(path: Optional[str] = None):
     lib.dann_shards_search_batch.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp]
     lib.dann_shards_free.argtypes = [vp]
     lib.dann_shards_free.restype = None
+    lib.dann_shards_scan_begin.argtypes = [vp, C.POINTER(vp)]
+    lib.dann_shards_scan_rescan.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int]
+    lib.dann_shards_scan_gettuple.argtypes = [vp, u32p, C.POINTER(C.c_uint16), u32p, C.POINTER(C.c_float),
+                                              C.POINTER(C.c_int32)]
+    lib.dann_shards_scan_stats.argtypes = [vp, C.POINTER(_QueryStats)]
+    lib.dann_shards_scan_end.argtypes = [vp]
+    lib.dann_shards_scan_end.restype = None
     lib.dann_coalescer_create.argtypes = [vp, C.c_int, C.c_int, C.POINTER(vp)]
     lib.dann_coalescer_search.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp]
     lib.dann_coalescer_gettuple.argtypes = [vp, vp, u32p, C.POINTER(C.c_uint16), u32p, C.POINTER(C.c_float)]
@@ -557,6 +566,10 @@ class ShardedIndex:
         h = self._lib.dann_shards_index(self._h, int(i))
         return DiskAnnIndex._view(self, h, self._geom[i], self.devices[i])
 
+    def begin_scan(self) -> "ShardedScan":
+        """ambeginscan over every shard: one streaming scan whose rows are the shards' scans merged."""
+        return ShardedScan(self)
+
     def search_batch(self, queries, labels=None, k: int = 10, search_list_size: int = QUERY_SEARCH_LIST_SIZE_DEFAULT,
                      rescore: int = QUERY_RESCORE_DEFAULT) -> dict:
         """Merged first k rows of B queries over every shard: dict(tid[B,k], dist[B,k], shard[B,k] i32 (-1 past count),
@@ -589,6 +602,64 @@ class ShardedIndex:
     def __del__(self):
         try:
             self.close()
+        except Exception:
+            pass
+
+
+class ShardedScan:
+    """amrescan / amgettuple / amendscan over a sharded table (dann_shards_scan_*): one IndexScan per shard, merged one
+    row at a time by the rule of ShardedIndex.search_batch, so its first k rows are the batch's k rows.  The first
+    gettuple after a rescan steps every shard (the shards of one device in one launch round); each later call steps the
+    shard whose row the previous call returned."""
+
+    def __init__(self, index: ShardedIndex):
+        self._index = index
+        self._lib = index._lib
+        h = C.c_void_p()
+        _check(self._lib, self._lib.dann_shards_scan_begin(index._h, C.byref(h)))
+        self._h = h
+
+    def rescan(self, query, labels: Optional[Sequence[int]] = None,
+               search_list_size: int = QUERY_SEARCH_LIST_SIZE_DEFAULT,
+               rescore: int = QUERY_RESCORE_DEFAULT):
+        """amrescan on every shard, as IndexScan.rescan; rescore must be > 0."""
+        q = None if query is None else np.ascontiguousarray(query, dtype=np.float32)
+        if q is not None and q.shape != (self._index.dim,):
+            raise ValueError(f"query must have {self._index.dim} dimensions")
+        if labels is None:
+            lab, nl = None, -1
+        else:
+            lab = np.ascontiguousarray(list(labels), dtype=np.int16)
+            nl = int(lab.size)
+        _check(self._lib, self._lib.dann_shards_scan_rescan(
+            self._h, _np_ptr(q), _np_ptr(lab) if lab is not None and lab.size else None, nl,
+            int(search_list_size), int(rescore)))
+
+    def gettuple(self):
+        """amgettuple: next merged row as (block, offset, node_id, distance, shard) or None at end of scan; node_id is
+        local to its shard."""
+        b, o, n, d, s = C.c_uint32(), C.c_uint16(), C.c_uint32(), C.c_float(), C.c_int32()
+        rc = _check(self._lib, self._lib.dann_shards_scan_gettuple(self._h, C.byref(b), C.byref(o), C.byref(n),
+                                                                   C.byref(d), C.byref(s)))
+        if rc == 0:
+            return None
+        return int(b.value), int(o.value), int(n.value), float(d.value), int(s.value)
+
+    def stats(self) -> list:
+        """One dict per shard: that shard's scan counters (IndexScan.stats)."""
+        st = (_QueryStats * self._index.count)()
+        _check(self._lib, self._lib.dann_shards_scan_stats(self._h, st))
+        return [{k: int(getattr(x, k)) for k, _ in _QueryStats._fields_} for x in st]
+
+    def end(self):
+        """amendscan."""
+        if getattr(self, "_h", None):
+            self._lib.dann_shards_scan_end(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.end()
         except Exception:
             pass
 

@@ -89,13 +89,12 @@ def merge_ms(sh, q, L, rescore, calls=5):
     return round(sum(e.device_time for e in ev) / max(len(ev), 1) / 1e3, 4), len(ev)
 
 
-def run(n, S, devices, data, parity_queries, reps):
-    from oracle import oracle
+def build_sharded(n, S, devices, data, res):
+    """The table's S shards loaded, their graphs built and their rows attached, with B queries and the exact top-K of
+    each over the whole table -> (ShardedIndex, snapshots, each shard's global row ids, each shard's device rows,
+    queries on the first device, truth); None when it does not fit (res["error"] says why)."""
     from pgvectorscale_b200 import diskann
-    from shard_model import scan_shards
     dev0 = torch.device("cuda", devices[0])
-    res = {"shards": S, "devices": devices, "rows_per_shard": []}
-    t0 = time.time()
     parts = shard_chunks(n, S)
     snaps, gids = [], []
     for i in range(S):
@@ -134,8 +133,19 @@ def run(n, S, devices, data, parity_queries, reps):
             sh.close()
         X.clear()
         torch.cuda.empty_cache()
+        return None
+    return sh, snaps, gids, X, q, topk.result()
+
+
+def run(n, S, devices, data, parity_queries, reps):
+    from oracle import oracle
+    from shard_model import scan_shards
+    res = {"shards": S, "devices": devices, "rows_per_shard": []}
+    t0 = time.time()
+    built = build_sharded(n, S, devices, data, res)
+    if built is None:
         return res
-    truth = topk.result()
+    sh, snaps, gids, X, q, truth = built
     qh = q.cpu().numpy()
     res["fixture_s"] = round(time.time() - t0, 1)
 
