@@ -113,11 +113,18 @@ static int dann_make_plan(const PlanInputs &in, uint32_t nq, uint32_t L, uint32_
     if (in.allow_lean && !force_single && in.R <= 64 && !in.plain_dim && ((in.words + 1u) & ~1u) <= 192u &&
         env_u32("DANN_SEARCH_KERNEL", 3) == 3 && !small_batch) {
         /* inserted-set: bitmap over node ids while a node id fits the 21-bit payload of a 4-byte entry and the
-         * bitmap is not larger than the hash set; else an open-addressing set of 1.5 x the candidate bound
-         * (3 x under a label key: rejected ids are recorded too), any multiple of 4 slots */
-        const uint64_t hcap = ((uint64_t)p->cand_cap * (keyed ? 3u : 1u) * 3u / 2u + 3u) & ~3ull;
+         * bitmap is not larger than a hash set of 1.5 x the candidate bound (3 x under a label key: rejected ids are
+         * recorded too); else an open-addressing hash set, any multiple of 4 slots.  Without a key the table is twice
+         * that, 3 x the candidate bound, as far as a 4-byte entry can address its slots: the linear probes of a visit
+         * are dependent compare-and-swap rounds on its chain, and the warp waits for the longest of its ~50 ids, so a
+         * lower load factor takes rounds off every visit.  At the 20M x 768 headline point on an H100 the search
+         * launch took 54.1 / 49.2 / 48.2 / 47.6 / 47.8 ms with tables of 1 / 1.5 / 2 / 3 / 4.5 x the bound, with
+         * identical rows (profiles/h100_hash_table_size_20m.json): past 3 x, the larger clear of the table (an HBM
+         * write per query) takes back what the fewer rounds save. */
+        const uint64_t hmin = ((uint64_t)p->cand_cap * (keyed ? 3u : 1u) * 3u / 2u + 3u) & ~3ull;
+        const uint64_t hcap = keyed ? hmin : std::max<uint64_t>(hmin, std::min<uint64_t>(2u * hmin, 1u << 21));
         const uint64_t bm_bytes = (uint64_t)((in.n + 127u) / 128u) * 16u;
-        bool bm = in.n <= (1u << 21) && bm_bytes <= hcap * 4u;
+        bool bm = in.n <= (1u << 21) && bm_bytes <= hmin * 4u;
         if (getenv("DANN_SEARCH_BITMAP")) bm = env_u32("DANN_SEARCH_BITMAP", 0) != 0 && in.n <= (16u << 20);
         const bool small = maxdist < 2048 && (bm ? in.n <= (1u << 21) : hcap <= (1u << 21)) && p->cand_cap <= (1u << 21);
         int entry3 = small ? 0 : 2;
