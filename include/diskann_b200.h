@@ -125,11 +125,17 @@ int dann_scan_begin(dann_index *ix, dann_scan **out);
  * GUCs diskann.query_search_list_size / diskann.query_rescore (guc.rs:3-4). */
 int dann_scan_rescan(dann_scan *sc, const float *query, const int16_t *labels, int nlabels,
                      int search_list_size, int rescore);
-/* How far a scan may stream: the suspended search's workspace is planned for rescore + 64 streamed rows; a scan that
- * runs past it (a selective post-filter without LIMIT) has its workspace rebuilt twice as large and the stream
- * replayed from row 0 - invisible to the caller except in time (the k-th doubling replays 2^k x the first plan) - up
- * to eight doublings or 2^30 candidates per query, then DANN_ERR_CAPACITY.  The reference can stream the whole index
- * through amgettuple; this operator is built for top-k scans (k ~ rescore) and says so.
+/* How far a scan may stream: to the end of the index, as the reference's next_with_resort does, with exactly its rows,
+ * dist bits and dann_scan_stats after every call.  The only condition is device memory for the search state: a
+ * failed allocation returns DANN_ERR_OOM.  The suspended search's workspace is planned for rescore + 64 streamed rows;
+ * a scan that runs past it (a selective post-filter, or no LIMIT) has its workspace rebuilt twice as large and the
+ * stream replayed from row 0 - invisible to the caller except in time.  Where that planned workspace can grow no
+ * further (eight doublings in one call, or a visited list past shared memory, or 2^30 candidates) the scan enters the
+ * deep mode once: its search is rebuilt with 8-byte heap entries, an inserted-set bitmap over every node id (n / 8
+ * bytes) and the visited list in HBM, and replayed one last time.  From then on it suspends before a visit that
+ * might not fit, grows its buffers in place (at least twice as large, the live state copied on the device) and
+ * resumes the same step: no row is generated twice.  dann_scan_rescan returns the scan to the planned workspace and
+ * frees the deep buffers, as dann_scan_end does.  The batch entry points keep their bounds.
  * One amgettuple: resumes the scan's suspended search (its state lives in HBM between calls), pulls
  * exactly the rows TSVResponseIterator::next_with_resort would (scan.rs:244-305), pops one.
  * Returns 1 and fills the outputs for the next row, 0 at end of scan, <0 on error.
@@ -144,13 +150,22 @@ int dann_scan_gettuple(dann_scan *sc, uint32_t *block, uint16_t *offset, uint32_
  * plan and workspace), so the backends of a serving process share the GPU instead of queueing behind each other.
  * Returns DANN_OK, or before anything runs: DANN_ERR_INVALID_ARG for n outside 1..65536, a NULL scans / out_rc / scan,
  * scans of different indexes or a scan listed twice, DANN_ERR_STATE for a scan that has not been rescanned.  A scan
- * whose workspace cannot grow further gets DANN_ERR_CAPACITY in out_rc and leaves the others unaffected; so does one
- * whose buffers cannot be allocated (DANN_ERR_OOM).  Any other failure returns an error only while no scan has taken
+ * whose buffers cannot be allocated gets DANN_ERR_OOM in out_rc and leaves the others unaffected; a scan that must grow
+ * its workspace (by replay or, in the deep mode, in place) does so alone and rejoins the next round.  Any other failure returns an error only while no scan has taken
  * its step; once one has, it goes to out_rc of the scans it hit, and the rows of the others stand.  dann_last_error()
  * describes the last failure of the call, which need not be scan i's. */
 int dann_scan_gettuple_many(dann_scan *const *scans, int n, int32_t *out_rc, uint32_t *block, uint16_t *offset,
                             uint32_t *node_id, float *dist);
 int dann_scan_stats(dann_scan *sc, dann_query_stats *out);
+/* What a scan holds: its mode, how it got there since the last dann_scan_rescan, and the device memory it keeps. */
+typedef struct {
+    uint32_t mode;         /* 0 = the planned workspace, 1 = deep (see dann_scan_gettuple) */
+    uint32_t regrows;      /* replay regrows */
+    uint32_t growths;      /* in-place growths of the deep mode */
+    uint32_t reserved;     /* 0 */
+    uint64_t device_bytes; /* bytes of device memory held by the scan */
+} dann_scan_workspace_info;
+int dann_scan_workspace(dann_scan *sc, dann_scan_workspace_info *out);
 void dann_scan_end(dann_scan *sc);
 
 /* ---- entry points that take DEVICE buffers (dann_search_batch_device, dann_prepare_queries, dann_sbq_distance,

@@ -34,6 +34,9 @@
 #define DANN_ST_VIS 4u
 // the two-warp kernel's heap warp popped another node than the memory warp predicted (never retried: an internal error)
 #define DANN_ST_INTERNAL 8u
+// a deep scan (dann_make_deep_plan) suspended cleanly before a visit its workspace has no room for: the host grows the
+// workspace in place and resumes the same step; no overflow happened and the saved state is valid
+#define DANN_ST_GROW 16u
 
 struct IndexView {
     uint32_t n, dim, dim_index, bits, words, cw, R, Rp;

@@ -21,6 +21,7 @@ struct SearchPlan {
     bool pairs; /* two-warp kernel (memory warp + heap warp per query) */
     bool lean;  /* dann_search3.cuh: one warp and a few KB of shared memory per query, up to 32 queries per SM */
     int maxw;   /* lean: the instantiation's resident-warp bound (32 -> 64 registers per thread, 16 -> 128) */
+    bool deep;  /* a streaming scan past what this plan's rule can give it (dann_make_deep_plan): the DEEP kernels */
 };
 
 /* what the plan depends on besides the request */
@@ -66,6 +67,7 @@ static int pick_code_mapping(uint32_t cw, uint32_t *G, uint32_t *Gshift, uint32_
 static int dann_make_plan(const PlanInputs &in, uint32_t nq, uint32_t L, uint32_t c_target, uint32_t grow, bool keyed,
                           SearchPlan *p, bool force_single, char *err, size_t errlen) {
     err[0] = 0;
+    p->deep = false;
     /* visits are about L + consumed; every visit stages at most R ids */
     uint64_t need = (((uint64_t)L + c_target) * 23 / 20 + 40u) * in.R * grow; /* 15% slack over L + consumed */
     /* test hook: start from a deliberately small workspace to exercise the growth path */
@@ -196,6 +198,33 @@ static int dann_make_plan(const PlanInputs &in, uint32_t nq, uint32_t L, uint32_
     p->per_warp = (uint32_t)((fixed + (size_t)hs * p->esize + 15) & ~(size_t)15);
     p->grid = std::min<uint32_t>((uint32_t)in.sm_count, (nq + W - 1) / W);
     return DANN_OK;
+}
+
+/* heap entries a deep scan keeps in shared memory: the top 10 levels.  A scan step copies them in and out (8 KB each
+ * way), so a larger top would tax every amgettuple of a deep scan to speed up only its pops. */
+#define DANN_DEEP_HS 1024u
+
+/* The deep plan of a streaming scan that has outgrown what dann_make_plan can give it: Ent64 entries (32-bit sequence
+ * numbers: the candidate count is bounded by n, not by the entry layout), an inserted-set bitmap over every node id
+ * (n / 8 bytes; it never fills up, so there is no inserted list and no rehash), the visited list in HBM, and a shared
+ * window of the heap top and the staging lists only.  cand_cap and vcap are the caller's: the scan grows them in place
+ * (dann_scan_gettuple), the heap top stays at DANN_DEEP_HS entries, so the heap's HBM tail keeps its positions. */
+static void dann_make_deep_plan(const PlanInputs &in, uint32_t cand_cap, uint32_t vcap, SearchPlan *p) {
+    *p = SearchPlan{};
+    p->cand_cap = (uint32_t)std::min<uint64_t>(((uint64_t)std::max(cand_cap, DANN_DEEP_HS) + 1023) & ~1023ull, 0xFFFFFC00u);
+    p->need = p->cand_cap;
+    p->vcap = (std::max<uint32_t>(vcap, 8u) + 3u) & ~3u;
+    p->bitmap_words = ((in.n + 127u) / 128u) * 4u;
+    p->hash_cap = 4u; /* unused */
+    p->ins_cap = 0;
+    p->entry = 2;
+    p->esize = 8;
+    p->hs = DANN_DEEP_HS;
+    p->W = 1;
+    p->grid = 1;
+    /* heap top + staging list + distances + the plain layout's query slice */
+    p->per_warp = (uint32_t)(((size_t)p->hs * 8 + 2 * DANN_LIST_CAP * 4 + (size_t)((in.plain_dim + 3u) & ~3u) * 4 + 15) & ~(size_t)15);
+    p->deep = true;
 }
 
 /* The launch arguments every search kernel takes from the index (its view, code mapping and list check) and from the

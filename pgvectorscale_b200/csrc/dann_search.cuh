@@ -20,7 +20,8 @@
 //
 // State placement
 //   shared : visited list (sorted, (dist<<32)|node), first `hs` heap entries, 64-entry
-//            staging list for one neighbour list.
+//            staging list for one neighbour list.  A deep scan (DEEP = 1) keeps its
+//            visited list in HBM instead.
 //   HBM    : per-warp workspace — inserted-set, seq->node table, heap tail beyond `hs`.
 //            The inserted-set is a bitmap over node ids (one atomicOr per neighbour, cleared
 //            by replaying the list of inserted ids) when the index is small enough for
@@ -40,11 +41,16 @@
 #include "dann_heap.cuh"
 
 /* PLAIN = 1: the plain storage layout.  Keys are total_ukey(f32 distance) (Ent64 entries), every comparison is a
- * full-distance comparison (counted as d_full), there is no label filter (plain/storage.rs:260). */
-template <typename T, int NCH, int PLAIN = 0>
+ * full-distance comparison (counted as d_full), there is no label filter (plain/storage.rs:260).
+ * DEEP = 1: a streaming scan's deep mode (dann_make_deep_plan, Ent64 only).  The visited list is saved_vis itself, in
+ * HBM; the inserted-set is a bitmap over every node id with no inserted list; the search suspends with DANN_ST_GROW
+ * before a visit that might not fit instead of overflowing.  Its own instantiations, so that the planned-workspace
+ * kernels keep their code. */
+template <typename T, int NCH, int PLAIN = 0, int DEEP = 0>
 struct SearchWarp {
     using E = typename T::E;
     using H = RustHeap<E, T::KSHIFT>;
+    static_assert(!DEEP || sizeof(E) == 8, "the deep scan mode has 8-byte heap entries");
     /* code rows gathered per lane group before reducing (16-B loads in flight = RPI*NCH):
      * with G=4 lanes per 192-B row, 8 x 8 rows = all 64 staged rows in one round */
     static constexpr int RPI = NCH <= 3 ? 8 : (NCH == 4 ? 4 : 2);
@@ -94,7 +100,9 @@ struct SearchWarp {
         const unsigned lt = (1u << lane) - 1u;
         const unsigned nm0 = __ballot_sync(DANN_FULL, new0), nm1 = __ballot_sync(DANN_FULL, new1);
         const uint32_t c0 = __popc(nm0), c1 = __popc(nm1);
-        if (a.bitmap_words) {
+        if (DEEP) { /* the bitmap spans every node id: it cannot fill up, and no inserted list is kept */
+            nins += c0 + c1;
+        } else if (a.bitmap_words) {
             if (nins + c0 + c1 > a.ins_cap) {
                 /* undo this round's bits so that the replay below leaves the bitmap all zero */
                 if (new0) atomicAnd(bitmap + (n0 >> 5), ~(1u << (n0 & 31)));
@@ -262,22 +270,27 @@ struct SearchWarp {
         }
     }
 
+    /* slide the visited window [vis_head, vis_head + vis_len) back to offset 0 */
+    __device__ __forceinline__ void visited_to_front() {
+        for (uint32_t i0 = 0; i0 < vis_len; i0 += 32) {
+            uint32_t i = i0 + lane;
+            uint64_t e = 0;
+            if (i < vis_len) e = vis[vis_head + i];
+            __syncwarp();
+            if (i < vis_len) vis[i] = e;
+            __syncwarp();
+        }
+        vis_head = 0;
+    }
+
     /* ---- visited.insert(partition_point(x < c), c) : graph/mod.rs:166-168 */
     __device__ __forceinline__ void visited_insert(uint32_t d, uint32_t node) {
-        if (vis_head + vis_len + 1 > a.vcap) { /* slide the window back to offset 0 */
+        if (vis_head + vis_len + 1 > a.vcap) {
             if (vis_len + 1 > a.vcap) {
                 status |= DANN_ST_VIS;
                 return;
             }
-            for (uint32_t i0 = 0; i0 < vis_len; i0 += 32) {
-                uint32_t i = i0 + lane;
-                uint64_t e = 0;
-                if (i < vis_len) e = vis[vis_head + i];
-                __syncwarp();
-                if (i < vis_len) vis[i] = e;
-                __syncwarp();
-            }
-            vis_head = 0;
+            visited_to_front();
         }
         uint64_t *w = vis + vis_head;
         uint32_t idx = 0;
@@ -316,7 +329,12 @@ struct SearchWarp {
             const E *hsrc = reinterpret_cast<const E *>(a.saved_heap_sm);
             const uint32_t hn = heap_len < heap.hs ? heap_len : heap.hs;
             for (uint32_t i = lane; i < hn; i += 32) heap.sm[i] = hsrc[i];
-            for (uint32_t i = lane; i < vis_len; i += 32) vis[i] = a.saved_vis[i];
+            if (DEEP) {
+                /* a step that suspended for growth (valid == 2) goes on appending after the rows it reported */
+                if (a.saved->valid == 2u) scount = a.stream_len[q];
+            } else {
+                for (uint32_t i = lane; i < vis_len; i += 32) vis[i] = a.saved_vis[i];
+            }
             __syncwarp();
         }
         if constexpr (PLAIN == 1) { /* the query's index slice, read by every distance of this scan */
@@ -368,6 +386,12 @@ struct SearchWarp {
                 }
                 go = __shfl_sync(DANN_FULL, go, 0);
                 if (!go) break;
+                /* deep scan: suspend at this visit boundary unless the visit surely fits - R candidates (hence R heap
+                 * slots and R seq->node entries) and one visited entry */
+                if (DEEP && (ncand + ix.R > a.cand_cap || vis_len + 1 > a.vcap)) {
+                    status = DANN_ST_GROW;
+                    break;
+                }
                 head = __shfl_sync(DANN_FULL, head, 0);
                 /* the popped element IS the current root: fetch its node id and neighbour list
                  * first, then let the sift-down and the visited insert run under that latency */
@@ -405,10 +429,15 @@ struct SearchWarp {
             E *hdst = reinterpret_cast<E *>(a.saved_heap_sm);
             const uint32_t hn = heap_len < heap.hs ? heap_len : heap.hs;
             for (uint32_t i = lane; i < hn; i += 32) hdst[i] = heap.sm[i];
-            for (uint32_t i = lane; i < vis_len; i += 32) a.saved_vis[i] = vis[vis_head + i];
+            if (DEEP) { /* the list already is saved_vis: just restart it at offset 0 */
+                if (vis_head) visited_to_front();
+            } else {
+                for (uint32_t i = lane; i < vis_len; i += 32) a.saved_vis[i] = vis[vis_head + i];
+            }
             if (lane == 0) {
                 SavedScan sv;
-                sv.valid = status ? 0u : 1u;
+                /* 2: suspended mid-step for growth, the step's rows so far in stream_len (written below) */
+                sv.valid = DEEP && status == DANN_ST_GROW ? 2u : status ? 0u : 1u;
                 sv.heap_len = heap_len;
                 sv.vis_len = vis_len;
                 sv.ncand = ncand;
@@ -430,13 +459,20 @@ struct SearchWarp {
 /* The warp's storage: its per_warp_smem layout at `base` (visited list, heap top, staging list, PLAIN query slice) and
  * workspace slot `slot` of the HBM arrays.  dann_search_kernel below carves the same layout inline: called from there,
  * this helper changes the order ptxas schedules that kernel in, and its measured SASS is kept as it is. */
-template <typename T, int NCH, int PLAIN>
-__device__ __forceinline__ void bind_search_warp(SearchWarp<T, NCH, PLAIN> &w, const SearchArgs &a, unsigned char *base,
+template <typename T, int NCH, int PLAIN, int DEEP>
+__device__ __forceinline__ void bind_search_warp(SearchWarp<T, NCH, PLAIN, DEEP> &w, const SearchArgs &a, unsigned char *base,
                                                  uint32_t slot) {
     using E = typename T::E;
-    w.vis = reinterpret_cast<uint64_t *>(base);
-    E *hsm = reinterpret_cast<E *>(base + (size_t)a.vcap * 8);
-    w.list = reinterpret_cast<uint32_t *>(base + (size_t)a.vcap * 8 + (size_t)a.hs * sizeof(E));
+    E *hsm;
+    if constexpr (DEEP) { /* the visited list lives in HBM (saved_vis): the shared window starts with the heap top */
+        w.vis = a.saved_vis;
+        hsm = reinterpret_cast<E *>(base);
+        w.list = reinterpret_cast<uint32_t *>(base + (size_t)a.hs * sizeof(E));
+    } else {
+        w.vis = reinterpret_cast<uint64_t *>(base);
+        hsm = reinterpret_cast<E *>(base + (size_t)a.vcap * 8);
+        w.list = reinterpret_cast<uint32_t *>(base + (size_t)a.vcap * 8 + (size_t)a.hs * sizeof(E));
+    }
     w.dl = w.list + DANN_LIST_CAP;
     w.qrow = reinterpret_cast<float *>(w.dl + DANN_LIST_CAP); /* PLAIN only: [plain_dim rounded up to 4] */
     w.hash = a.hash + (size_t)slot * a.hash_cap;
@@ -448,17 +484,24 @@ __device__ __forceinline__ void bind_search_warp(SearchWarp<T, NCH, PLAIN> &w, c
     w.heap.hs = a.hs;
 }
 
-template <typename T, int NCH, int PLAIN = 0>
+template <typename T, int NCH, int PLAIN = 0, int DEEP = 0>
 __global__ void __launch_bounds__(384, 1) dann_search_kernel(const SearchArgs a) {
     using E = typename T::E;
     DANN_DYN_SMEM(dann_smem);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, W = blockDim.x >> 5;
     const uint32_t slot = blockIdx.x * W + warp;
     unsigned char *base = dann_smem + (size_t)warp * a.per_warp_smem;
-    SearchWarp<T, NCH, PLAIN> w(a, lane);
-    w.vis = reinterpret_cast<uint64_t *>(base);
-    E *hsm = reinterpret_cast<E *>(base + (size_t)a.vcap * 8);
-    w.list = reinterpret_cast<uint32_t *>(base + (size_t)a.vcap * 8 + (size_t)a.hs * sizeof(E));
+    SearchWarp<T, NCH, PLAIN, DEEP> w(a, lane);
+    E *hsm;
+    if constexpr (DEEP) { /* as in bind_search_warp */
+        w.vis = a.saved_vis;
+        hsm = reinterpret_cast<E *>(base);
+        w.list = reinterpret_cast<uint32_t *>(base + (size_t)a.hs * sizeof(E));
+    } else {
+        w.vis = reinterpret_cast<uint64_t *>(base);
+        hsm = reinterpret_cast<E *>(base + (size_t)a.vcap * 8);
+        w.list = reinterpret_cast<uint32_t *>(base + (size_t)a.vcap * 8 + (size_t)a.hs * sizeof(E));
+    }
     w.dl = w.list + DANN_LIST_CAP;
     w.qrow = reinterpret_cast<float *>(w.dl + DANN_LIST_CAP); /* PLAIN only: [plain_dim rounded up to 4] */
     w.hash = a.hash + (size_t)slot * a.hash_cap;
@@ -479,7 +522,7 @@ __global__ void __launch_bounds__(384, 1) dann_search_kernel(const SearchArgs a)
  * dann_scan_gettuple clears with a memset before its launch.  Register budget: 168 per thread, the one
  * dann_search_kernel's (384, 1) bound gives the same code (with a bare 32-thread bound ptxas settles on 128 for some
  * Ent64 instantiations and spills). */
-template <typename T, int NCH, int PLAIN = 0>
+template <typename T, int NCH, int PLAIN = 0, int DEEP = 0>
 __global__ void __launch_bounds__(32, 12) dann_scan_search_many_kernel(const SearchArgs *args, uint32_t nscans) {
     DANN_DYN_SMEM(dann_smem);
     DANN_STATIC_SMEM __align__(16) unsigned char s_args[sizeof(SearchArgs)];
@@ -493,7 +536,7 @@ __global__ void __launch_bounds__(32, 12) dann_scan_search_many_kernel(const Sea
     const SearchArgs &a = *reinterpret_cast<const SearchArgs *>(s_args);
     if (lane == 0) *a.overflow = 0u;
     __syncwarp();
-    SearchWarp<T, NCH, PLAIN> w(a, lane);
+    SearchWarp<T, NCH, PLAIN, DEEP> w(a, lane);
     bind_search_warp(w, a, dann_smem, 0u);
     w.run(0u);
 }

@@ -141,6 +141,25 @@ struct DevBuf {
         if (e == cudaSuccess) cap = want;
         return e;
     }
+    /* reserve() that keeps bytes [from, to) of the old contents: copied device to device on `st`, which is then
+     * synchronised, before the old allocation goes */
+    cudaError_t grow_keep(size_t bytes, size_t from, size_t to, cudaStream_t st) {
+        if (bytes <= cap) return cudaSuccess;
+        void *q = nullptr;
+        const size_t want = bytes + bytes / 4 + 256;
+        cudaError_t e = cudaMalloc(&q, want);
+        if (e != cudaSuccess) return e;
+        if (to > from) e = cudaMemcpyAsync((char *)q + from, (const char *)p + from, to - from, cudaMemcpyDeviceToDevice, st);
+        if (e == cudaSuccess) e = cudaStreamSynchronize(st);
+        if (e != cudaSuccess) {
+            cudaFree(q);
+            return e;
+        }
+        if (p) cudaFree(p);
+        p = q;
+        cap = want;
+        return cudaSuccess;
+    }
     void release() {
         if (p) cudaFree(p);
         p = nullptr;
@@ -206,6 +225,9 @@ struct dann_scan {
         d_ins, d_stream, d_slen, d_stats, d_dist, d_win, d_winst, d_ctl;
     SearchPlan plan{};
     uint32_t grow = 1;
+    bool deep = false;      /* plan is the deep plan (dann_make_deep_plan): the workspace grows in place */
+    uint32_t regrows = 0;   /* replay regrows since the rescan */
+    uint32_t growths = 0;   /* in-place growths since the rescan */
     uint32_t streamed = 0;  /* rows taken off the approximate stream so far */
     uint32_t win_len = 0;   /* rows sitting in the rerank window */
     bool exhausted = false; /* next() returned None */
@@ -605,14 +627,14 @@ extern "C" int dann_full_distance(dann_index *ix, const float *d_q_full, const u
 /* ------------------------------------------------------------------------------------ */
 /* search kernel dispatch                                                                */
 typedef void (*search_fn)(const SearchArgs);
-template <typename T>
+template <typename T, int DEEP = 0>
 static search_fn pick_search(uint32_t nch) {
     switch (nch) {
-        case 1: return dann_search_kernel<T, 1>;
-        case 2: return dann_search_kernel<T, 2>;
-        case 3: return dann_search_kernel<T, 3>;
-        case 4: return dann_search_kernel<T, 4>;
-        default: return dann_search_kernel<T, 8>;
+        case 1: return dann_search_kernel<T, 1, 0, DEEP>;
+        case 2: return dann_search_kernel<T, 2, 0, DEEP>;
+        case 3: return dann_search_kernel<T, 3, 0, DEEP>;
+        case 4: return dann_search_kernel<T, 4, 0, DEEP>;
+        default: return dann_search_kernel<T, 8, 0, DEEP>;
     }
 }
 template <typename T>
@@ -625,7 +647,8 @@ static search_fn pick_search2(uint32_t nch) {
         default: return dann_search2_kernel<T, 8>;
     }
 }
-static search_fn pick_kernel(bool pairs, int entry, uint32_t nch, bool plain = false) {
+static search_fn pick_kernel(bool pairs, int entry, uint32_t nch, bool plain = false, bool deep = false) {
+    if (deep) return plain ? dann_search_kernel<Ent64, 1, 1, 1> : pick_search<Ent64, 1>(nch); /* the deep plan: Ent64 */
     if (plain) return dann_search_kernel<Ent64, 1, 1>;
     if (pairs) return entry == 0 ? pick_search2<Ent32x21>(nch) : entry == 1 ? pick_search2<Ent32x16>(nch) : pick_search2<Ent64>(nch);
     return entry == 0 ? pick_search<Ent32x21>(nch) : entry == 1 ? pick_search<Ent32x16>(nch) : pick_search<Ent64>(nch);
@@ -633,17 +656,18 @@ static search_fn pick_kernel(bool pairs, int entry, uint32_t nch, bool plain = f
 
 /* dann_scan_search_many_kernel: the instantiations pick_kernel(false, ...) offers the streaming scan */
 typedef void (*scan_many_fn)(const SearchArgs *, uint32_t);
-template <typename T>
+template <typename T, int DEEP = 0>
 static scan_many_fn pick_scan_many_t(uint32_t nch) {
     switch (nch) {
-        case 1: return dann_scan_search_many_kernel<T, 1>;
-        case 2: return dann_scan_search_many_kernel<T, 2>;
-        case 3: return dann_scan_search_many_kernel<T, 3>;
-        case 4: return dann_scan_search_many_kernel<T, 4>;
-        default: return dann_scan_search_many_kernel<T, 8>;
+        case 1: return dann_scan_search_many_kernel<T, 1, 0, DEEP>;
+        case 2: return dann_scan_search_many_kernel<T, 2, 0, DEEP>;
+        case 3: return dann_scan_search_many_kernel<T, 3, 0, DEEP>;
+        case 4: return dann_scan_search_many_kernel<T, 4, 0, DEEP>;
+        default: return dann_scan_search_many_kernel<T, 8, 0, DEEP>;
     }
 }
-static scan_many_fn pick_scan_many(int entry, uint32_t nch, bool plain) {
+static scan_many_fn pick_scan_many(int entry, uint32_t nch, bool plain, bool deep) {
+    if (deep) return plain ? dann_scan_search_many_kernel<Ent64, 1, 1, 1> : pick_scan_many_t<Ent64, 1>(nch);
     if (plain) return dann_scan_search_many_kernel<Ent64, 1, 1>;
     return entry == 0 ? pick_scan_many_t<Ent32x21>(nch) : entry == 1 ? pick_scan_many_t<Ent32x16>(nch) : pick_scan_many_t<Ent64>(nch);
 }
@@ -1242,10 +1266,13 @@ extern "C" int dann_scan_begin(dann_index *ix, dann_scan **out) try {
     return DANN_OK;
 } DANN_CATCH
 
+#define DANN_SCAN_BUFS(sc)                                                                                               \
+    {&(sc)->d_qindex, &(sc)->d_step, &(sc)->d_query, &(sc)->d_qfull, &(sc)->d_qcodes, &(sc)->d_labels, &(sc)->d_label_off, \
+     &(sc)->d_saved, &(sc)->d_heap_sm, &(sc)->d_vis, &(sc)->d_heap_tail, &(sc)->d_cnode, &(sc)->d_set, &(sc)->d_ins,       \
+     &(sc)->d_stream, &(sc)->d_slen, &(sc)->d_stats, &(sc)->d_dist, &(sc)->d_win, &(sc)->d_winst, &(sc)->d_ctl}
+
 static void scan_release(dann_scan *sc) {
-    DevBuf *bufs[] = {&sc->d_qindex, &sc->d_step, &sc->d_query, &sc->d_qfull, &sc->d_qcodes, &sc->d_labels, &sc->d_label_off, &sc->d_saved,
-                      &sc->d_heap_sm, &sc->d_vis, &sc->d_heap_tail, &sc->d_cnode, &sc->d_set, &sc->d_ins, &sc->d_stream,
-                      &sc->d_slen, &sc->d_stats, &sc->d_dist, &sc->d_win, &sc->d_winst, &sc->d_ctl};
+    DevBuf *bufs[] = DANN_SCAN_BUFS(sc);
     for (DevBuf *b : bufs) b->release();
 }
 
@@ -1301,6 +1328,13 @@ static int scan_rescan_enqueue(dann_scan *sc, const float *query, const int16_t 
     sc->L = search_list_size;
     sc->rescore = rescore;
     sc->grow = 1;
+    if (sc->deep) { /* back to the planned workspace: give the deep scan's buffers back (reserve() never shrinks) */
+        DevBuf *deep_bufs[] = {&sc->d_heap_sm, &sc->d_vis, &sc->d_heap_tail, &sc->d_cnode, &sc->d_set, &sc->d_ins,
+                               &sc->d_stream, &sc->d_dist};
+        for (DevBuf *b : deep_bufs) b->release();
+        sc->deep = false;
+    }
+    sc->regrows = sc->growths = 0;
     sc->streamed = sc->win_len = 0;
     sc->exhausted = false;
     sc->stats = dann_query_stats{};
@@ -1398,7 +1432,7 @@ static int scan_launch_search(dann_scan *sc, uint32_t want) {
     int rc = scan_search_args(sc, want, &a);
     if (rc) return rc;
     CK(cudaMemsetAsync(sc->d_ctl.p, 0, 8, st));
-    search_fn fn = pick_kernel(false, p.entry, ix->NCH, ix->plain);
+    search_fn fn = pick_kernel(false, p.entry, ix->NCH, ix->plain, p.deep);
     CK(cudaFuncSetAttribute(fn, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(p.per_warp + DANN_SMEM_SLACK)));
     fn<<<1, 32, p.per_warp + DANN_SMEM_SLACK, st>>>(a);
     ix->launches++;
@@ -1442,12 +1476,76 @@ static ScanFinishDesc scan_finish_desc(dann_scan *sc, bool searching, uint32_t s
     return f;
 }
 
-/* the scan outgrew its workspace: rebuild it twice as large (its reset enqueued on `st`, the stream its next search
- * runs on); the next search replays the stream up to sc->streamed */
+/* Rebuild the scan's suspended search as the deep plan, with the candidate and visited capacity of the planned workspace
+ * it leaves (its reset enqueued on `st`); the next search replays the stream up to sc->streamed, once, and grows the
+ * workspace in place wherever that replay or a later step needs more (scan_grow_in_place). */
+static int scan_enter_deep(dann_scan *sc, cudaStream_t st) {
+    dann_index *ix = sc->ix;
+    PlanInputs in{};
+    in.n = ix->v.n;
+    in.R = ix->v.R;
+    in.plain_dim = ix->plain ? ix->v.dim_index : 0;
+    /* the start nodes of a label key are staged before any visit: room for all of them and one visit */
+    const uint64_t cand = std::max<uint64_t>(sc->plan.cand_cap, (uint64_t)sc->labels.size() + ix->v.R);
+    SearchPlan &p = sc->plan;
+    dann_make_deep_plan(in, (uint32_t)std::min<uint64_t>(cand, 0xFFFFFC00u), sc->plan.vcap, &p);
+    sc->deep = true;
+    sc->d_ins.release();
+    CK(sc->d_saved.reserve(sizeof(SavedScan)));
+    CK(sc->d_heap_sm.reserve((size_t)p.hs * p.esize + 16));
+    CK(sc->d_vis.reserve((size_t)p.vcap * 8));
+    CK(sc->d_heap_tail.reserve((size_t)p.cand_cap * p.esize));
+    CK(sc->d_cnode.reserve((size_t)p.cand_cap * 4));
+    CK(sc->d_set.reserve((size_t)p.bitmap_words * 4));
+    CK(cudaMemsetAsync(sc->d_set.p, 0, (size_t)p.bitmap_words * 4, st));
+    CK(cudaMemsetAsync(sc->d_saved.p, 0, sizeof(SavedScan), st));
+    return DANN_OK;
+}
+
+/* The scan outgrew its workspace: rebuild it twice as large (its reset enqueued on `st`, the stream its next search
+ * runs on); the next search replays the stream up to sc->streamed.  Where the planned workspace can grow no further -
+ * an eighth regrow in one call, or a plan dann_make_plan refuses - the scan enters the deep mode instead
+ * (DANN_DEBUG_DEEP_AFTER = k, a test hook: after k regrows of the scan). */
 static int scan_regrow(dann_scan *sc, int attempt, cudaStream_t st) {
-    if (attempt >= 8) return fail(DANN_ERR_CAPACITY, "scan workspace still too small after %d growth steps", attempt);
-    sc->grow *= 2;
-    return scan_reset_search(sc, st);
+    if (sc->deep) /* a deep scan suspends before it could overflow (DANN_ST_GROW) */
+        return fail(DANN_ERR_STATE, "internal error: a deep scan overflowed its workspace");
+    if (attempt < 8 && sc->regrows < env_u32("DANN_DEBUG_DEEP_AFTER", UINT32_MAX)) {
+        const SearchPlan last = sc->plan;
+        sc->grow *= 2;
+        const int rc = scan_reset_search(sc, st);
+        if (rc != DANN_ERR_CAPACITY) {
+            sc->regrows += rc == DANN_OK;
+            return rc;
+        }
+        sc->plan = last;
+    }
+    return scan_enter_deep(sc, st);
+}
+
+/* A deep scan suspended before a visit its workspace might not fit (DANN_ST_GROW): at least double what lacks room,
+ * keeping the live prefix of each array - the heap's HBM tail [hs, heap_len) (SplitStore indexes it by absolute
+ * position), the seq->node table [0, ncand) and the visited list [0, vis_len) - so that the same step resumes where it
+ * stopped.  The inserted-set bitmap and the heap top keep their size. */
+static int scan_grow_in_place(dann_scan *sc, cudaStream_t st) {
+    dann_index *ix = sc->ix;
+    SearchPlan &p = sc->plan;
+    SavedScan sv;
+    CK(cudaMemcpyAsync(&sv, sc->d_saved.p, sizeof sv, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    uint32_t cand = p.cand_cap, vcap = p.vcap;
+    if ((uint64_t)sv.ncand + ix->v.R > cand)
+        cand = (uint32_t)std::min<uint64_t>((std::max<uint64_t>(2ull * cand, (uint64_t)sv.ncand + ix->v.R) + 1023) & ~1023ull, 0xFFFFFC00u);
+    if (sv.vis_len + 1ull > vcap) vcap = (uint32_t)std::min<uint64_t>(2ull * vcap, 0xFFFFFFFCu);
+    if (cand == p.cand_cap && vcap == p.vcap)
+        return fail(DANN_ERR_STATE, "internal error: a deep scan suspended with room for its next visit");
+    const size_t hs_bytes = (size_t)p.hs * 8, tail_end = (size_t)sv.heap_len * 8;
+    CK(sc->d_heap_tail.grow_keep((size_t)cand * 8, hs_bytes, std::max(tail_end, hs_bytes), st));
+    CK(sc->d_cnode.grow_keep((size_t)cand * 4, 0, (size_t)sv.ncand * 4, st));
+    CK(sc->d_vis.grow_keep((size_t)vcap * 8, 0, (size_t)sv.vis_len * 8, st));
+    p.cand_cap = p.need = cand;
+    p.vcap = vcap;
+    sc->growths++;
+    return DANN_OK;
 }
 
 /* The host side of a step that did not overflow: the stream position, end of stream and counters of the scan, then its
@@ -1491,7 +1589,7 @@ extern "C" int dann_scan_gettuple(dann_scan *sc, uint32_t *block, uint16_t *offs
     const bool searching = need && !sc->exhausted;
     ScanStepOut o;
     uint32_t skip = 0; /* rows that are only re-generated because the workspace had to grow */
-    for (int attempt = 0;; attempt++) {
+    for (int attempt = 0;;) {
         const uint32_t want = skip + need;
         if (searching) {
             rc = scan_launch_search(sc, want);
@@ -1515,7 +1613,12 @@ extern "C" int dann_scan_gettuple(dann_scan *sc, uint32_t *block, uint16_t *offs
         CK(cudaMemcpyAsync(&o, sc->d_step.p, sizeof o, cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
         if (!o.overflow) break;
-        rc = scan_regrow(sc, attempt, st);
+        if (o.overflow == DANN_ST_GROW) { /* the same step resumes after the rows it already appended */
+            rc = scan_grow_in_place(sc, st);
+            if (rc) return rc;
+            continue;
+        }
+        rc = scan_regrow(sc, attempt++, st);
         if (rc) return rc;
         skip = sc->streamed;
     }
@@ -1648,7 +1751,7 @@ static int scan_gettuple_many_locked(dann_index *lead, dann_scan *const *scans, 
         searchers.clear();
         for (Step *s : round)
             if (s->searching) {
-                s->fn = pick_scan_many(s->sc->plan.entry, s->sc->ix->NCH, s->sc->ix->plain);
+                s->fn = pick_scan_many(s->sc->plan.entry, s->sc->ix->NCH, s->sc->ix->plain, s->sc->plan.deep);
                 searchers.push_back(s);
             }
         std::stable_sort(searchers.begin(), searchers.end(),
@@ -1697,12 +1800,13 @@ static int scan_gettuple_many_locked(dann_index *lead, dann_scan *const *scans, 
                 moved = true;
                 continue;
             }
-            rc = scan_regrow(s->sc, s->attempt++, lead->stream);
-            if (rc) { /* capacity, memory, or a CUDA error that has poisoned the handle: this scan alone */
+            const bool grow = outs[j].overflow == DANN_ST_GROW; /* a deep scan resumes its step where it stopped */
+            rc = grow ? scan_grow_in_place(s->sc, lead->stream) : scan_regrow(s->sc, s->attempt++, lead->stream);
+            if (rc) { /* memory, or a CUDA error that has poisoned the handle: this scan alone */
                 scan_failed(s, rc);
                 continue;
             }
-            s->skip = s->sc->streamed;
+            if (!grow) s->skip = s->sc->streamed;
             next.push_back(s);
         }
         round.swap(next);
@@ -1742,6 +1846,17 @@ extern "C" int dann_scan_gettuple_many(dann_scan *const *scans, int n, int32_t *
 extern "C" int dann_scan_stats(dann_scan *sc, dann_query_stats *out) try {
     if (!sc || !out) return fail(DANN_ERR_INVALID_ARG, "dann_scan_stats: NULL argument");
     *out = sc->stats;
+    return DANN_OK;
+} DANN_CATCH
+
+extern "C" int dann_scan_workspace(dann_scan *sc, dann_scan_workspace_info *out) try {
+    if (!sc || !out) return fail(DANN_ERR_INVALID_ARG, "dann_scan_workspace: NULL argument");
+    *out = dann_scan_workspace_info{};
+    out->mode = sc->deep ? 1u : 0u;
+    out->regrows = sc->regrows;
+    out->growths = sc->growths;
+    const DevBuf *bufs[] = DANN_SCAN_BUFS(sc);
+    for (const DevBuf *b : bufs) out->device_bytes += b->cap;
     return DANN_OK;
 } DANN_CATCH
 

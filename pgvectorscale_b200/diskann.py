@@ -66,6 +66,11 @@ class _QueryStats(C.Structure):
                 ("d_full", C.c_uint32), ("stream_len", C.c_uint32), ("status", C.c_uint32)]
 
 
+class _ScanWorkspace(C.Structure):
+    _fields_ = [("mode", C.c_uint32), ("regrows", C.c_uint32), ("growths", C.c_uint32), ("reserved", C.c_uint32),
+                ("device_bytes", C.c_uint64)]
+
+
 STATS_DTYPE = np.dtype([("visits", "<u4"), ("d_quantized", "<u4"), ("candidates", "<u4"),
                         ("d_full", "<u4"), ("stream_len", "<u4"), ("status", "<u4")])
 
@@ -74,7 +79,7 @@ EXPORTS = [
     "dann_last_error", "dann_device_count", "dann_index_load", "dann_index_load_plain", "dann_index_free",
     "dann_coalescer_create", "dann_coalescer_search", "dann_coalescer_stats", "dann_coalescer_destroy",
     "dann_index_hbm_bytes", "dann_scan_begin", "dann_scan_rescan", "dann_scan_gettuple", "dann_scan_gettuple_many",
-    "dann_coalescer_gettuple", "dann_scan_stats", "dann_scan_end", "dann_search_batch", "dann_search_batch_device",
+    "dann_coalescer_gettuple", "dann_scan_stats", "dann_scan_workspace", "dann_scan_end", "dann_search_batch", "dann_search_batch_device",
     "dann_prepare_queries", "dann_code_stride", "dann_sbq_distance", "dann_full_distance",
     "dann_kernel_launches", "dann_last_batch_timing",
     "dann_build_graph", "dann_index_download_nbrs", "dann_index_set_vectors", "dann_index_set_vectors_device",
@@ -119,6 +124,7 @@ def load_library(path: Optional[str] = None):
     lib.dann_scan_gettuple.argtypes = [vp, u32p, C.POINTER(C.c_uint16), u32p, C.POINTER(C.c_float)]
     lib.dann_scan_gettuple_many.argtypes = [vp, C.c_int, vp, vp, vp, vp, vp]
     lib.dann_scan_stats.argtypes = [vp, C.POINTER(_QueryStats)]
+    lib.dann_scan_workspace.argtypes = [vp, C.POINTER(_ScanWorkspace)]
     lib.dann_scan_end.argtypes = [vp]
     lib.dann_scan_end.restype = None
     lib.dann_search_batch.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp]
@@ -439,6 +445,13 @@ class IndexScan:
         st = _QueryStats()
         _check(self._lib, self._lib.dann_scan_stats(self._h, C.byref(st)))
         return {k: int(getattr(st, k)) for k, _ in _QueryStats._fields_}
+
+    def workspace(self) -> dict:
+        """What the scan holds (dann_scan_workspace): mode (0 = planned workspace, 1 = deep), regrows (replay regrows)
+        and growths (in-place growths) since the last rescan, device_bytes held."""
+        w = _ScanWorkspace()
+        _check(self._lib, self._lib.dann_scan_workspace(self._h, C.byref(w)))
+        return {k: int(getattr(w, k)) for k in ("mode", "regrows", "growths", "device_bytes")}
 
     def end(self):
         """amendscan."""
