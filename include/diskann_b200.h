@@ -196,6 +196,38 @@ int dann_search_batch_device(dann_index *ix, const float *d_queries, const int16
                              uint32_t *d_out_count, dann_query_stats *d_out_stats,
                              void *stream);
 
+/* ---- batch whose queries differ in k, search_list_size, rescore and key ---------------------------------------
+ * One query's request.  `params` is a host array [B] for the host entry points and a device array for _device. */
+typedef struct {
+    int32_t k;                /* rows wanted, >= 1 */
+    int32_t search_list_size; /* 1..10000, guc.rs:11-26 */
+    int32_t rescore;          /* 0..1000,  guc.rs:28-43 */
+    int32_t keyed;            /* 0 = no scan key (labels None); 1 = labels[label_off[b] .. label_off[b+1]) */
+} dann_query_params;
+/* B independent scans in one launch of each kernel, each with its own parameters.
+ * - Output: rows are [B][kmax] with kmax the largest params[b].k; query b's rows start at b * kmax.  Past out_count[b]
+ *   (at most params[b].k) a row holds DANN_INVALID_TID and NaN.
+ * - Per query: query b gets exactly what a dann_search_batch of that query alone returns with its own k,
+ *   search_list_size, rescore and key - tids, distance bits, out_count and every dann_query_stats field - whatever it
+ *   is batched with, and through any workspace-growth reruns.
+ * - Keys: keyed = 0 is no key, and its label_off range must be empty.  keyed = 1 with an empty range is
+ *   `labels && ARRAY[]`, which returns no rows.  label_off may be NULL only when no query is keyed.  The host entry
+ *   point sorts and deduplicates each key, as dann_search_batch does; the device entry point needs sorted keys.
+ * - Checks, all before anything runs (DANN_ERR_INVALID_ARG, the message names the query; the handle stays usable):
+ *   B < 1, a NULL params, a value out of range, keyed not 0 or 1, a non-monotone label_off, a keyed query without
+ *   label_off, a query whose own k and rescore exceed the rerank kernel's shared memory (the dann_search_batch rule).
+ * - Plain layout: a keyed query is refused, and a query's rescore counts as 0 when dim == dim_index.
+ * The plan is made for the batch's largest search_list_size and stream, and for a key if any query has one.
+ * dann_search_batch_mixed_device reads params (and label_off) back to check them, then runs as
+ * dann_search_batch_device does. */
+int dann_search_batch_mixed(dann_index *ix, const float *queries, const int16_t *labels, const int32_t *label_off,
+                            const dann_query_params *params, int B, uint64_t *out_tid, float *out_dist,
+                            uint32_t *out_count, dann_query_stats *out_stats);
+int dann_search_batch_mixed_device(dann_index *ix, const float *d_queries, const int16_t *d_labels,
+                                   const int32_t *d_label_off, const dann_query_params *d_params, int B,
+                                   uint64_t *d_out_tid, float *d_out_dist, uint32_t *d_out_count,
+                                   dann_query_stats *d_out_stats, void *stream);
+
 /* ---- stand-alone kernels (roofline metric + per-kernel parity tests), device buffers -- */
 /* amrescan's vector preparation: cosine-normalise + SBQ-quantize B queries.
  * d_q_full [B*dim] (may be NULL), d_q_codes [B*dann_code_stride(ix)]. */
@@ -250,6 +282,11 @@ dann_index *dann_group_replica(dann_group *g, int i); /* replica i (e.g. to atta
 int dann_group_search_batch(dann_group *g, const float *queries, const int16_t *labels, const int32_t *label_offsets,
                             int B, int k, int search_list_size, int rescore, uint64_t *out_tid, float *out_dist,
                             uint32_t *out_count, dann_query_stats *out_stats);
+/* dann_search_batch_mixed over the replicas: params is sliced with the queries, rows are [B][kmax] of the whole batch,
+ * and the whole batch is checked before any replica runs. */
+int dann_group_search_batch_mixed(dann_group *g, const float *queries, const int16_t *labels, const int32_t *label_off,
+                                  const dann_query_params *params, int B, uint64_t *out_tid, float *out_dist,
+                                  uint32_t *out_count, dann_query_stats *out_stats);
 void dann_group_free(dann_group *g);
 
 /* ---- a table split into shards: one independent index per shard, one merged top-k per query -------------------
@@ -415,9 +452,10 @@ int dann_last_search_plan(dann_index *ix, dann_search_plan_info *out);
  * Postgres is process-per-connection with amcanparallel = false (mod.rs:63): one scan per backend at a time, while
  * the engine's throughput comes from batches.  A coalescer owns a dispatcher thread; any number of host threads (one
  * per connected backend in a sidecar that holds the HBM-resident index) call dann_coalescer_search with ONE query and
- * block; requests that arrive within max_wait_us of the first one (at most max_batch, same k / search_list_size /
- * rescore, all keyed or all unkeyed) become one dann_search_batch call.  Each caller receives exactly the rows,
- * distances and counters a private dann_search_batch of its query returns.  nlabels < 0 = no scan key.
+ * block; the search requests that arrive within max_wait_us of the first one (at most max_batch, whatever their k,
+ * search_list_size, rescore and key) become one dann_search_batch_mixed call.  Each caller receives exactly the rows,
+ * distances and counters a private dann_search_batch of its query returns.  nlabels < 0 = no scan key.  A request the
+ * index would refuse (a value out of range, a rescore past the rerank window) is refused at once, for its caller alone.
  * The socket / shared-memory transport between backends and the sidecar is not part of this library. */
 typedef struct dann_coalescer dann_coalescer;
 int dann_coalescer_create(dann_index *ix, int max_batch, int max_wait_us, dann_coalescer **out);

@@ -4,8 +4,9 @@
 // index scan in flight, one query at a time, while the GPU reaches its throughput on batches (one query = one warp
 // pair).  The coalescer is the piece a sidecar that owns the HBM-resident index would put between the two: any number
 // of host threads (one per connected backend) submit single queries and block; a dispatcher thread gathers what
-// arrives within a short window into ONE dann_search_batch call and hands every caller its own rows.  Queries are
-// independent units, so each caller gets exactly what a private scan would have returned.
+// arrives within a short window into ONE dann_search_batch_mixed call and hands every caller its own rows.  Queries are
+// independent units, whatever their k, search_list_size, rescore or key, so each caller gets exactly what a private
+// scan would have returned.
 // The same dispatcher coalesces amgettuple calls: the gettuple requests of a window (any scans of the index, whatever
 // their search_list_size, rescore or key) become ONE dann_scan_gettuple_many call, and each caller gets the row its
 // own dann_scan_gettuple would have returned.  Search and gettuple requests never share a dispatch.
@@ -50,10 +51,8 @@ struct dann_coalescer {
     uint64_t n_batches = 0, n_queries = 0, max_seen = 0;
 
     static bool compatible(const CoalescedRequest *a, const CoalescedRequest *b) {
-        /* gettuple requests all go into one dann_scan_gettuple_many call */
-        if (a->scan || b->scan) return a->scan && b->scan;
-        /* one dann_search_batch call shares k / L / rescore and is either all keyed or all unkeyed */
-        return a->k == b->k && a->L == b->L && a->rescore == b->rescore && (a->nlabels >= 0) == (b->nlabels >= 0);
+        /* gettuple requests all go into one dann_scan_gettuple_many call, search requests into one mixed batch */
+        return (a->scan != nullptr) == (b->scan != nullptr);
     }
 
     void run() {
@@ -81,7 +80,7 @@ struct dann_coalescer {
                     batch.push_back(*it); /* reserved above: does not allocate */
                     it = queue.erase(it);
                 } else {
-                    ++it; /* different scan parameters: next window */
+                    ++it; /* the other kind of request: next window */
                 }
             }
             lk.unlock();
@@ -117,35 +116,38 @@ struct dann_coalescer {
         if (batch[0]->scan) return execute_gettuple(batch);
         const int B = (int)batch.size();
         const uint32_t dim = ix->v.dim;
-        const int k = batch[0]->k;
-        const bool keyed = batch[0]->nlabels >= 0;
         std::vector<float> q((size_t)B * dim);
         std::vector<int16_t> lab;
-        std::vector<int32_t> off;
-        for (int b = 0; b < B; b++) memcpy(q.data() + (size_t)b * dim, batch[b]->query, (size_t)dim * sizeof(float));
-        if (keyed) {
-            off.assign(1, 0);
-            for (int b = 0; b < B; b++) {
-                lab.insert(lab.end(), batch[b]->labels, batch[b]->labels + batch[b]->nlabels);
-                off.push_back((int32_t)lab.size());
-            }
-            if (lab.empty()) lab.push_back(0);
+        std::vector<int32_t> off(1, 0);
+        std::vector<dann_query_params> params((size_t)B);
+        for (int b = 0; b < B; b++) {
+            const CoalescedRequest *r = batch[b];
+            memcpy(q.data() + (size_t)b * dim, r->query, (size_t)dim * sizeof(float));
+            if (r->nlabels > 0) lab.insert(lab.end(), r->labels, r->labels + r->nlabels);
+            off.push_back((int32_t)lab.size());
+            params[(size_t)b] = dann_query_params{r->k, r->L, r->rescore, r->nlabels >= 0 ? 1 : 0};
         }
+        if (lab.empty()) lab.push_back(0);
+        /* each request was checked on its own at submission, so the batch is refused only if the index is */
+        int rc = check_live(ix);
+        BatchParams bp;
+        if (!rc) rc = mixed_params(ix, B, params.data(), lab.data(), off.data(), 0, &bp);
+        const int k = bp.k;
         std::vector<uint64_t> tid((size_t)B * k);
         std::vector<float> dist((size_t)B * k);
         std::vector<uint32_t> count(B);
         std::vector<dann_query_stats> stats(B);
-        const int rc = search_batch_host(ix, q.data(), keyed ? lab.data() : nullptr, keyed ? off.data() : nullptr, B, k,
-                                         batch[0]->L, batch[0]->rescore, tid.data(), dist.data(), nullptr, count.data(),
-                                         stats.data());
+        if (!rc)
+            rc = search_batch_host(ix, q.data(), lab.data(), off.data(), B, bp, tid.data(), dist.data(), nullptr, count.data(),
+                                   stats.data());
         const std::string err = rc ? g_err : std::string();
         for (int b = 0; b < B; b++) {
             CoalescedRequest *r = batch[b];
             r->rc = rc;
             r->err = err;
             if (rc) continue;
-            memcpy(r->out_tid, tid.data() + (size_t)b * k, (size_t)k * sizeof(uint64_t));
-            if (r->out_dist) memcpy(r->out_dist, dist.data() + (size_t)b * k, (size_t)k * sizeof(float));
+            memcpy(r->out_tid, tid.data() + (size_t)b * k, (size_t)r->k * sizeof(uint64_t));
+            if (r->out_dist) memcpy(r->out_dist, dist.data() + (size_t)b * k, (size_t)r->k * sizeof(float));
             if (r->out_count) *r->out_count = count[b];
             if (r->out_stats) *r->out_stats = stats[b];
         }
@@ -238,6 +240,11 @@ extern "C" int dann_coalescer_search(dann_coalescer *c, const float *query, cons
                                      uint32_t *out_count, dann_query_stats *out_stats) try {
     if (!c || !query || !out_tid || k <= 0) return fail(DANN_ERR_INVALID_ARG, "dann_coalescer_search: bad argument");
     if (nlabels > 0 && !labels) return fail(DANN_ERR_INVALID_ARG, "labels is NULL but nlabels > 0");
+    /* a request the index would refuse is refused here, for this caller alone: the rest of its window goes ahead */
+    int checked_rescore = rescore;
+    size_t smem = 0;
+    const int rc = check_query(c->ix, "", k, search_list_size, &checked_rescore, nlabels >= 0, &smem);
+    if (rc) return rc;
     CoalescedRequest r;
     r.query = query;
     r.labels = labels;

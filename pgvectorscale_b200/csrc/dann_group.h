@@ -97,6 +97,7 @@ struct dann_group {
     const int16_t *labels = nullptr;
     const int32_t *label_off = nullptr;
     int k = 0, L = 0, rescore = 0;
+    const dann_query_params *params = nullptr; /* dann_group_search_batch_mixed; k is then the whole batch's row stride */
     uint32_t dim = 0;
     uint64_t *out_tid = nullptr;
     float *out_dist = nullptr;
@@ -106,9 +107,19 @@ struct dann_group {
     int run(size_t i) {
         const int l = lo[i], h = hi[i];
         if (h <= l) return DANN_OK;
-        return search_batch_host(ix[i], queries + (size_t)l * dim, labels, label_off ? label_off + l : nullptr, h - l, k, L,
-                                 rescore, out_tid + (size_t)l * k, out_dist ? out_dist + (size_t)l * k : nullptr, nullptr,
-                                 out_count ? out_count + l : nullptr, out_stats ? out_stats + l : nullptr);
+        const float *q = queries + (size_t)l * dim;
+        const int32_t *off = label_off ? label_off + l : nullptr;
+        uint64_t *tid = out_tid + (size_t)l * k;
+        float *dist = out_dist ? out_dist + (size_t)l * k : nullptr;
+        uint32_t *count = out_count ? out_count + l : nullptr;
+        dann_query_stats *stats = out_stats ? out_stats + l : nullptr;
+        if (!params) return search_batch_host(ix[i], q, labels, off, h - l, k, L, rescore, tid, dist, nullptr, count, stats);
+        /* the slice's own parameters, with the rows laid out at the whole batch's stride */
+        int rc = check_live(ix[i]);
+        if (rc) return rc;
+        BatchParams bp;
+        rc = mixed_params(ix[i], h - l, params + l, labels, off, k, &bp);
+        return rc ? rc : search_batch_host(ix[i], q, labels, off, h - l, bp, tid, dist, nullptr, count, stats);
     }
 };
 
@@ -154,17 +165,12 @@ extern "C" dann_index *dann_group_replica(dann_group *g, int i) {
     return (g && i >= 0 && (size_t)i < g->ix.size()) ? g->ix[(size_t)i] : nullptr;
 }
 
-extern "C" int dann_group_search_batch(dann_group *g, const float *queries, const int16_t *labels, const int32_t *label_off,
-                                       int B, int k, int search_list_size, int rescore, uint64_t *out_tid, float *out_dist,
-                                       uint32_t *out_count, dann_query_stats *out_stats) try {
-    if (!g || B <= 0 || k <= 0 || !queries || !out_tid) return fail(DANN_ERR_INVALID_ARG, "dann_group_search_batch: bad argument");
-    std::lock_guard<std::mutex> one(g->call_mu);
+/* one batch call over the replicas; the caller holds call_mu and has set k / L / rescore / params */
+static int group_call(dann_group *g, int B, const float *queries, const int16_t *labels, const int32_t *label_off,
+                      uint64_t *out_tid, float *out_dist, uint32_t *out_count, dann_query_stats *out_stats) {
     g->queries = queries;
     g->labels = labels;
     g->label_off = label_off;
-    g->k = k;
-    g->L = search_list_size;
-    g->rescore = rescore;
     g->out_tid = out_tid;
     g->out_dist = out_dist;
     g->out_count = out_count;
@@ -175,4 +181,31 @@ extern "C" int dann_group_search_batch(dann_group *g, const float *queries, cons
     for (int r = 0; r < world; r++)
         if (g->loop.w[(size_t)r].rc) return fail(g->loop.w[(size_t)r].rc, "replica %d: %s", r, g->loop.w[(size_t)r].err.c_str());
     return DANN_OK;
+}
+
+extern "C" int dann_group_search_batch(dann_group *g, const float *queries, const int16_t *labels, const int32_t *label_off,
+                                       int B, int k, int search_list_size, int rescore, uint64_t *out_tid, float *out_dist,
+                                       uint32_t *out_count, dann_query_stats *out_stats) try {
+    if (!g || B <= 0 || k <= 0 || !queries || !out_tid) return fail(DANN_ERR_INVALID_ARG, "dann_group_search_batch: bad argument");
+    std::lock_guard<std::mutex> one(g->call_mu);
+    g->params = nullptr;
+    g->k = k;
+    g->L = search_list_size;
+    g->rescore = rescore;
+    return group_call(g, B, queries, labels, label_off, out_tid, out_dist, out_count, out_stats);
+} DANN_CATCH
+
+/* The slices are those of dann_group_search_batch, params sliced with the queries; the whole batch is checked on replica
+ * 0 first (the replicas are copies of one index), so a refused batch runs nowhere. */
+extern "C" int dann_group_search_batch_mixed(dann_group *g, const float *queries, const int16_t *labels, const int32_t *label_off,
+                                             const dann_query_params *params, int B, uint64_t *out_tid, float *out_dist,
+                                             uint32_t *out_count, dann_query_stats *out_stats) try {
+    if (!g || !queries || !out_tid) return fail(DANN_ERR_INVALID_ARG, "dann_group_search_batch_mixed: bad argument");
+    BatchParams bp;
+    int rc = mixed_params(g->ix[0], B, params, labels, label_off, 0, &bp);
+    if (rc) return rc;
+    std::lock_guard<std::mutex> one(g->call_mu);
+    g->params = params;
+    g->k = bp.k;
+    return group_call(g, B, queries, labels, label_off, out_tid, out_dist, out_count, out_stats);
 } DANN_CATCH

@@ -131,9 +131,10 @@ __global__ void __launch_bounds__(128) dann_prepare_plain_kernel(uint32_t dim, u
 /* Plain storage layout, after the rerank kernel: every comparison of the beam search was a full-distance comparison
  * (plain/storage.rs:238,288), so d_full = candidates + reranked rows and d_quantized = 0.  Only launched when the
  * rerank ran (num_dimensions_to_index < num_dimensions, scan.rs:392-403). */
-__global__ void dann_plain_stats_kernel(dann_query_stats *stats, int B) {
+__global__ void dann_plain_stats_kernel(dann_query_stats *stats, int B, const QueryParam *qp = nullptr) {
     const int q = blockIdx.x * blockDim.x + threadIdx.x;
     if (q >= B) return;
+    if (qp && qp[q].rescore == 0u) return; /* a query that reranks nothing keeps its search counters */
     dann_query_stats st = stats[q];
     st.d_full = st.candidates + st.d_full; /* the rerank kernel left the number of reranked rows here */
     st.d_quantized = 0;
@@ -296,6 +297,10 @@ struct RerankArgs {
     uint32_t *out_node;         /* [B][k] or NULL */
     uint32_t *out_count;        /* [B] or NULL */
     dann_query_stats *stats;    /* [B] or NULL : d_full is filled here */
+    /* per-query k, rescore and c_target (NULL = the three above apply to every query).  When set, c_target and k above
+     * are the row strides of the stream and the outputs, the batch maxima, and query q's rows past its own k are
+     * filled like the rows past its count.  Kept last. */
+    const QueryParam *qp = nullptr;
 };
 
 __global__ void __launch_bounds__(128) dann_rerank_kernel(const RerankArgs a) {
@@ -303,23 +308,28 @@ __global__ void __launch_bounds__(128) dann_rerank_kernel(const RerankArgs a) {
     const IndexView &ix = a.ix;
     float *qs = reinterpret_cast<float *>(dann_smem);                    /* [dim rounded to 4] */
     const uint32_t dim4 = (ix.dim + 3u) & ~3u;
-    float *ds = qs + dim4;                                              /* [c_target] */
-    uint64_t *hp = reinterpret_cast<uint64_t *>(ds + ((a.c_target + 1u) & ~1u)); /* [rescore] */
-    DANN_STATIC_SMEM uint64_t bar;
     const int q = blockIdx.x;
+    /* this query's k, rescore and stream length: its CTA lays out shared memory for its own sizes */
+    const uint32_t rescore = a.qp ? a.qp[q].rescore : a.rescore;
+    const uint32_t ctq = a.qp ? a.qp[q].c_target : a.c_target;
+    float *ds = qs + dim4;                                              /* [ctq] */
+    uint64_t *hp = reinterpret_cast<uint64_t *>(ds + ((ctq + 1u) & ~1u)); /* [rescore] */
+    DANN_STATIC_SMEM uint64_t bar;
     const uint32_t sl = a.stream_len[q];
     const uint32_t *st = a.stream + (size_t)q * a.c_target;
     uint64_t *otid = a.out_tid + (size_t)q * a.k;
 
-    if (a.rescore == 0) {
+    if (rescore == 0) {
+        const uint32_t kq = a.qp ? a.qp[q].k : a.k;
+        const uint32_t rows = sl < kq ? sl : kq;
         for (uint32_t i = threadIdx.x; i < a.k; i += blockDim.x) {
-            bool ok = i < sl;
+            bool ok = i < rows;
             uint32_t node = ok ? st[i] : DANN_INVALID_NODE;
             otid[i] = ok ? ix.tids[node] : DANN_INVALID_TID;
             if (a.out_dist) a.out_dist[(size_t)q * a.k + i] = DANN_NAN_F;
             if (a.out_node) a.out_node[(size_t)q * a.k + i] = node;
         }
-        if (threadIdx.x == 0 && a.out_count) a.out_count[q] = sl < a.k ? sl : a.k;
+        if (threadIdx.x == 0 && a.out_count) a.out_count[q] = rows;
         return;
     }
 
@@ -329,9 +339,11 @@ __global__ void __launch_bounds__(128) dann_rerank_kernel(const RerankArgs a) {
     if (threadIdx.x == 0) {
         using H = RustHeap<uint64_t, 32>;
         ArrayStore<uint64_t> store{hp};
+        /* read again rather than held across the distance phase (which would cost a spill) */
+        const uint32_t kq = a.qp ? a.qp[q].k : a.k, window = a.qp ? a.qp[q].rescore : a.rescore;
         uint32_t len = 0, si = 0, rows = 0;
-        for (; rows < a.k; rows++) {
-            while (len < a.rescore && si < sl) { /* refill: resort_buffer.push(ResortData{..}) */
+        for (; rows < kq; rows++) {
+            while (len < window && si < sl) { /* refill: resort_buffer.push(ResortData{..}) */
                 H::push(store, len, ((uint64_t)total_ukey(ds[si]) << 32) | si);
                 si++;
             }

@@ -356,7 +356,7 @@ struct SearchWarp {
         key = query_labels(a, q);
         /* greedy_search_streaming_init + ListSearchResult::new (graph/mod.rs:97-124,331-354) */
         if (ix.start_default != DANN_INVALID_NODE && !resumed) {
-            if (a.q_label_off) {
+            if (query_keyed(a, q)) {
                 for (uint32_t b = 0; b < key.n && !status; b += 32) {
                     uint32_t n;
                     const bool valid = label_start_node(ix, key, b + lane, n);
@@ -379,8 +379,9 @@ struct SearchWarp {
                 if (lane == 0 && heap_len > 0) { /* visit_closest, graph/mod.rs:153-170 */
                     head = heap.get(0);
                     go = 1;
-                    if (vis_len > a.L) {
-                        uint64_t at = vis[vis_head + a.L - 1];
+                    const uint32_t Lq = query_L(a, q);
+                    if (vis_len > Lq) {
+                        uint64_t at = vis[vis_head + Lq - 1];
                         if (H::key(head) >= (uint32_t)(at >> 32)) go = 0;
                     }
                 }
@@ -422,7 +423,7 @@ struct SearchWarp {
             if ((tid & 0xFFFFull) == 0) continue;       /* InvalidOffsetNumber: deleted tuple, scan.rs:231-234 */
             if (lane == 0) a.stream[(size_t)q * a.c_target + scount] = node;
             scount++;
-            if (scount == a.c_target) done = true;
+            if (scount == query_c_target(a, q)) done = true;
         }
         if (a.saved) { /* suspend: the inserted-set and the heap tail stay where they are */
             __syncwarp();

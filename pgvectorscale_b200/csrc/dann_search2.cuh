@@ -244,7 +244,8 @@ struct PairSearch {
         filter = false;
         uint32_t nstart_pages = 1;
         const bool have_graph = ix.start_default != DANN_INVALID_NODE;
-        if (a.q_label_off) {
+        const bool keyed = query_keyed(a, q);
+        if (keyed) {
             int32_t o0 = a.q_label_off[q], o1 = a.q_label_off[q + 1];
             ql = a.q_labels + o0;
             nql = (uint32_t)(o1 - o0);
@@ -259,7 +260,7 @@ struct PairSearch {
             uint32_t *list = listp + p * DANN_LIST_CAP, *dl = dlp + p * DANN_LIST_CAP;
             listn = 0;
             if (have_graph && !status) {
-                if (a.q_label_off) {
+                if (keyed) {
                     uint32_t n[2];
                     bool v[2];
 #pragma unroll
@@ -326,7 +327,7 @@ struct PairSearch {
             while (!status) {
                 /* visit_closest (graph/mod.rs:153-170): candidates empty -> None; strictly more than L
                  * visited and head >= visited[L-1] -> None; else pop */
-                if (have && !(vis_len > a.L && key >= (uint32_t)(vis[vis_head + a.L - 1] >> 32))) {
+                if (have && !(vis_len > query_L(a, q) && key >= (uint32_t)(vis[vis_head + query_L(a, q) - 1] >> 32))) {
                     visit = true;
                     break;
                 }
@@ -346,7 +347,7 @@ struct PairSearch {
                 if ((tid & 0xFFFFull) == 0) continue;     /* InvalidOffsetNumber: deleted tuple, scan.rs:231-234 */
                 if (lane == 0) a.stream[(size_t)q * a.c_target + scount] = cn;
                 scount++;
-                if (scount == a.c_target) break;
+                if (scount == query_c_target(a, q)) break;
             }
             if (!visit) { /* the scan is over (enough rows, stream exhausted, or a workspace overflow) */
                 if (lane == 0) ctl->cmd[p] = 0u;
@@ -517,7 +518,7 @@ struct PairSearch {
     __device__ __forceinline__ void run_heap(uint32_t q) {
         heap_len = hk = 0;
         uint32_t nstart_pages = 1;
-        if (a.q_label_off) {
+        if (query_keyed(a, q)) {
             uint32_t nql_ = (uint32_t)(a.q_label_off[q + 1] - a.q_label_off[q]);
             nstart_pages = nql_ ? (nql_ + 63) / 64 : 1;
         }

@@ -57,6 +57,7 @@ struct LeanWarp {
     QueryLabels key;
     bool slotpay;
     uint32_t heap_len, vis_head, vis_len, nset, listn, visits, dq, status;
+    uint32_t Lq; /* the query's search_list_size */
 
     __device__ __forceinline__ LeanWarp(const SearchArgs &a_, int lane_) : a(a_), lane(lane_) {}
 
@@ -533,8 +534,8 @@ struct LeanWarp {
 
     /* visit_closest's test (graph/mod.rs:153-170) for a candidate root */
     __device__ __forceinline__ bool may_visit(E head) const {
-        if (vis_len > a.L) {
-            const E at = vis[vix(a.L - 1)];
+        if (vis_len > Lq) {
+            const E at = vis[vix(Lq - 1)];
             if ((head | KM) >= (at | KM)) return false; /* head >= node_at_pos */
         }
         return true;
@@ -604,6 +605,8 @@ struct LeanWarp {
         visits = dq = status = 0;
         uint32_t scount = 0;
         slotpay = SMALL && a.bitmap_words == 0;
+        Lq = query_L(a, q);
+        const uint32_t ctq = query_c_target(a, q);
         { /* the query's SBQ code (SbqSearchDistanceMeasure, sbq/mod.rs:139-159) into shared memory: lane group member gl
            * compares chunks gl, gl + G, ... of every row against the same chunks of the query */
             const uint32_t nchunks = ix.cw >> 1, padded = (uint32_t)NCH * a.G;
@@ -615,7 +618,7 @@ struct LeanWarp {
         key = query_labels(a, q);
         /* greedy_search_streaming_init + ListSearchResult::new (graph/mod.rs:97-124,331-354) */
         if (ix.start_default != DANN_INVALID_NODE) {
-            if (a.q_label_off) {
+            if (query_keyed(a, q)) {
                 for (uint32_t b = 0; b < key.n && !status; b += 32) {
                     uint32_t n;
                     const bool valid = label_start_node(ix, key, b + lane, n);
@@ -661,7 +664,7 @@ struct LeanWarp {
             if ((tid & 0xFFFFull) == 0) continue;       /* InvalidOffsetNumber: deleted tuple, scan.rs:231-234 */
             if (lane == 0) a.stream[(size_t)q * a.c_target + scount] = node;
             scount++;
-            if (scount == a.c_target) done = true;
+            if (scount == ctq) done = true;
         }
         if (slotpay) dann_cp_async_wait_all(); /* no copy of this query's root node id outlives it */
         if (a.bitmap_words) { /* leave the bitmap all zero for the slot's next query */

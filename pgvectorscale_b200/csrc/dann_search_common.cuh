@@ -12,6 +12,13 @@ struct SavedScan {
     uint32_t valid, heap_len, vis_len, ncand, nins, visits, dq, exhausted;
 };
 
+/* One query's own parameters in a batch whose queries differ in them (dann_search_batch_mixed): its search_list_size,
+ * its stream length (c_target = k, or rescore + k - 1), whether it has a scan key, its k and its rescore (0 on a plain
+ * index that reranks nothing).  The launch's scalars hold the batch maxima. */
+struct QueryParam {
+    uint32_t L, c_target, keyed, k, rescore;
+};
+
 /* Index- and plan-derived fields are filled by search_args_for_plan (dann_plan.h); each launch adds its request, its
  * buffers and its mode.  Everything it leaves alone is null or zero. */
 struct SearchArgs {
@@ -60,6 +67,9 @@ struct SearchArgs {
     const float *plain_vectors = nullptr; /* [n][plain_dim] */
     const float *q_index = nullptr;       /* [B][plain_dim] prepared (truncated, cosine-normalised) queries */
     uint32_t plain_dim = 0;               /* num_dimensions_to_index */
+    /* per-query L, c_target and key (indexed by query id, after the qlist mapping); NULL = L, c_target and q_label_off
+     * above apply to every query.  The stream's row stride stays c_target, the batch maximum.  Kept last. */
+    const QueryParam *qp = nullptr;
 };
 #define DANN_HV_POP 2u
 
@@ -100,7 +110,14 @@ __device__ __forceinline__ void serve_queries(const SearchArgs &a, int lane, War
     }
 }
 
-/* the query's scan key: its labels, sorted and deduplicated (none when the launch has no q_label_off: labels None) */
+/* query q's search_list_size, stream length, and whether it has a scan key (labels None when it has not) */
+__device__ __forceinline__ uint32_t query_L(const SearchArgs &a, uint32_t q) { return a.qp ? a.qp[q].L : a.L; }
+__device__ __forceinline__ uint32_t query_c_target(const SearchArgs &a, uint32_t q) { return a.qp ? a.qp[q].c_target : a.c_target; }
+__device__ __forceinline__ bool query_keyed(const SearchArgs &a, uint32_t q) {
+    return a.q_label_off != nullptr && (!a.qp || a.qp[q].keyed != 0u);
+}
+
+/* the query's scan key: its labels, sorted and deduplicated (none when the query is unkeyed: labels None) */
 struct QueryLabels {
     const int16_t *l;
     uint32_t n;
@@ -108,7 +125,7 @@ struct QueryLabels {
 };
 __device__ __forceinline__ QueryLabels query_labels(const SearchArgs &a, uint32_t q) {
     QueryLabels k{nullptr, 0u, false};
-    if (a.q_label_off) {
+    if (query_keyed(a, q)) {
         const int32_t o0 = a.q_label_off[q], o1 = a.q_label_off[q + 1];
         k.l = a.q_labels + o0;
         k.n = (uint32_t)(o1 - o0);

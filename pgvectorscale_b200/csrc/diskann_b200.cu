@@ -187,6 +187,7 @@ struct dann_index {
     DevBuf sc_qfull, sc_qcodes, sc_stream, sc_stream_len, sc_stats, sc_qlist, sc_ctl, sc_node;
     /* staging for the host-buffer entry point */
     DevBuf st_queries, st_labels, st_label_off, st_tid, st_dist, st_count, st_stats;
+    DevBuf sc_qparams; /* a mixed batch's QueryParam per query */
     dann_batch_timing timing{};
     dann_search_plan_info last_plan{};
     cudaEvent_t ev[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};
@@ -297,7 +298,7 @@ extern "C" void dann_index_free(dann_index *ix) {
     DevBuf *bufs[] = {&ix->ws_hash, &ix->ws_cand, &ix->ws_heap, &ix->ws_bitmap, &ix->ws_ins, &ix->sc_qfull, &ix->sc_qcodes,
                       &ix->sc_stream, &ix->sc_stream_len, &ix->sc_stats, &ix->sc_qlist, &ix->sc_ctl,
                       &ix->sc_node, &ix->sc_qindex, &ix->st_queries, &ix->st_labels, &ix->st_label_off, &ix->st_tid,
-                      &ix->st_dist, &ix->st_count, &ix->st_stats, &ix->sc_many};
+                      &ix->st_dist, &ix->st_count, &ix->st_stats, &ix->sc_many, &ix->sc_qparams};
     for (DevBuf *b : bufs) b->release();
     for (auto &e : ix->ev)
         if (e) cudaEventDestroy(e);
@@ -730,7 +731,8 @@ static int make_plan(dann_index *ix, uint32_t nq, uint32_t L, uint32_t c_target,
  * vis_out != NULL selects build mode (dann_build.cuh). */
 static int run_search(dann_index *ix, const uint64_t *d_q_codes, const int16_t *d_labels, const int32_t *d_label_off,
                       int B, uint32_t L, uint32_t c_target, dann_query_stats *d_stats, uint64_t *vis_out,
-                      uint32_t *vis_out_len, uint32_t vis_out_cap, cudaStream_t st, const float *d_q_index = nullptr) {
+                      uint32_t *vis_out_len, uint32_t vis_out_cap, cudaStream_t st, const float *d_q_index = nullptr,
+                      const QueryParam *d_qp = nullptr) {
     const IndexView &v = ix->v;
     uint32_t *d_ctl = ix->sc_ctl.as<uint32_t>(); /* [0]=work counter, [1]=overflow bits */
     int rc;
@@ -781,6 +783,7 @@ static int run_search(dann_index *ix, const uint64_t *d_q_codes, const int16_t *
         a.plain_vectors = ix->index_vectors;
         a.q_index = d_q_index;
         a.plain_dim = ix->plain ? v.dim_index : 0;
+        a.qp = d_qp;
         if (attempt == 0) {
             dann_search_plan_info &pi = ix->last_plan;
             pi.kernel = p.lean ? 3u : p.pairs ? 2u : 1u;
@@ -836,30 +839,113 @@ static int run_search(dann_index *ix, const uint64_t *d_q_codes, const int16_t *
     return DANN_OK;
 }
 
-/* B queries, first k rows each.  All pointers are device pointers. */
+/* What a batch asks of its queries, checked and derived before anything runs.  A uniform batch (one k, L and rescore;
+ * keyed when label_off is given) leaves qp empty.  A mixed batch (dann_search_batch_mixed) holds each query's own values
+ * in qp, and k / L / rescore / c_target are the batch maxima: k is the row stride of the outputs, c_target that of the
+ * stream.  rerank_smem is the largest single query's rerank window. */
+struct BatchParams {
+    int k = 0, L = 0, rescore = 0;
+    uint32_t c_target = 0;
+    size_t rerank_smem = 0;
+    bool keyed = false; /* label_off goes to the kernels */
+    std::vector<QueryParam> qp;
+};
+
+/* rows needed from the approximate stream: scan.rs:255-305 */
+static uint32_t stream_rows(int k, int rescore) { return rescore == 0 ? (uint32_t)k : (uint32_t)rescore + (uint32_t)k - 1u; }
+
+/* One query's k, search_list_size and rescore (`who` names it in the messages): the GUC ranges, the plain layout's rules
+ * and the rerank kernel's shared memory.  *rescore becomes what the query reranks; *smem its rerank window. */
+static int check_query(const dann_index *ix, const char *who, int k, int L, int *rescore, bool keyed, size_t *smem) {
+    const IndexView &v = ix->v;
+    if (k <= 0) return fail(DANN_ERR_INVALID_ARG, "%sk %d must be positive", who, k);
+    if (L < 1 || L > 10000) return fail(DANN_ERR_INVALID_ARG, "%ssearch_list_size %d outside 1..10000 (guc.rs:11-26)", who, L);
+    if (*rescore < 0 || *rescore > 1000) return fail(DANN_ERR_INVALID_ARG, "%srescore %d outside 0..1000 (guc.rs:28-43)", who, *rescore);
+    if (ix->plain) {
+        if (keyed) return fail(DANN_ERR_INVALID_ARG, "%splain storage does not support label filters (plain/storage.rs:260)", who);
+        /* scan.rs:392-403: a plain index only resorts when it holds fewer dimensions than the heap column */
+        if (v.dim == v.dim_index) *rescore = 0;
+    }
+    if (*rescore > 0 && v.n && !v.vectors)
+        return fail(DANN_ERR_STATE, "%sindex has no heap vectors yet (dann_index_set_vectors): rescore must be 0", who);
+    /* the rerank kernel keeps the query row, one f32 per streamed row and the window in shared memory; a request past
+     * the limit is refused here, because a failed launch would poison the handle */
+    *smem = rerank_smem_bytes(v.dim, stream_rows(k, *rescore), (uint32_t)*rescore);
+    if (*smem > ix->rerank_smem_max)
+        return fail(DANN_ERR_INVALID_ARG, "%sk=%d rows with rescore=%d need %zu B of shared memory per scan (limit %zu): "
+                    "fetch fewer rows per scan", who, k, *rescore, *smem, ix->rerank_smem_max);
+    return DANN_OK;
+}
+
+static int uniform_params(const dann_index *ix, int B, int k, int L, int rescore, bool keyed, BatchParams *bp) {
+    if (B <= 0 || k <= 0) return fail(DANN_ERR_INVALID_ARG, "B and k must be positive");
+    int rc = check_query(ix, "", k, L, &rescore, keyed, &bp->rerank_smem);
+    if (rc) return rc;
+    bp->k = k;
+    bp->L = L;
+    bp->rescore = rescore;
+    bp->c_target = stream_rows(k, rescore);
+    bp->keyed = keyed;
+    bp->qp.clear();
+    return DANN_OK;
+}
+
+/* The checks of dann_search_batch_mixed, on host copies of params [B] and label_off [B+1] (NULL: no query keyed).
+ * kstride > 0 asks for that output row stride (a group slice writes into the whole batch's rows), else it is the largest
+ * k.  Nothing is touched on the device. */
+static int mixed_params(const dann_index *ix, int B, const dann_query_params *params, const int16_t *labels,
+                        const int32_t *label_off, int kstride, BatchParams *bp) {
+    if (B <= 0) return fail(DANN_ERR_INVALID_ARG, "B %d must be positive", B);
+    if (!params) return fail(DANN_ERR_INVALID_ARG, "params is NULL");
+    if (label_off && label_off[0] < 0) return fail(DANN_ERR_INVALID_ARG, "label_off[0] is negative");
+    bp->qp.resize((size_t)B);
+    bp->k = bp->L = bp->rescore = 0;
+    bp->c_target = 0;
+    bp->rerank_smem = 0;
+    bp->keyed = false;
+    for (int b = 0; b < B; b++) {
+        const dann_query_params &p = params[b];
+        char who[32];
+        snprintf(who, sizeof who, "query %d: ", b);
+        if (p.keyed != 0 && p.keyed != 1) return fail(DANN_ERR_INVALID_ARG, "%skeyed %d is not 0 or 1", who, p.keyed);
+        if (p.keyed && !label_off) return fail(DANN_ERR_INVALID_ARG, "%skeyed, but label_off is NULL", who);
+        if (label_off) {
+            const int32_t o0 = label_off[b], o1 = label_off[b + 1];
+            if (o1 < o0) return fail(DANN_ERR_INVALID_ARG, "%slabel_off is not monotone", who);
+            if (!p.keyed && o1 > o0) return fail(DANN_ERR_INVALID_ARG, "%sunkeyed (keyed = 0), but its label_off range is not empty", who);
+            if (o1 > o0 && !labels) return fail(DANN_ERR_INVALID_ARG, "%slabels is NULL but its key is not empty", who);
+        }
+        int rescore = p.rescore;
+        size_t smem = 0;
+        int rc = check_query(ix, who, p.k, p.search_list_size, &rescore, p.keyed != 0, &smem);
+        if (rc) return rc;
+        QueryParam &q = bp->qp[(size_t)b];
+        q.L = (uint32_t)p.search_list_size;
+        q.c_target = stream_rows(p.k, rescore);
+        q.keyed = (uint32_t)p.keyed;
+        q.k = (uint32_t)p.k;
+        q.rescore = (uint32_t)rescore;
+        bp->k = std::max(bp->k, p.k);
+        bp->L = std::max(bp->L, p.search_list_size);
+        bp->rescore = std::max(bp->rescore, rescore);
+        bp->c_target = std::max(bp->c_target, q.c_target);
+        bp->rerank_smem = std::max(bp->rerank_smem, smem);
+        bp->keyed = bp->keyed || p.keyed;
+    }
+    if (kstride > 0) bp->k = std::max(bp->k, kstride);
+    return DANN_OK;
+}
+
+/* B queries, the first k rows each (the first qp[b].k of a mixed batch).  All pointers are device pointers; d_labels /
+ * d_label_off are used when bp.keyed. */
 static int search_batch_device_locked(dann_index *ix, const float *d_queries, const int16_t *d_labels,
-                                      const int32_t *d_label_off, int B, int k, int L, int rescore,
+                                      const int32_t *d_label_off, int B, const BatchParams &bp,
                                       uint64_t *d_out_tid, float *d_out_dist, uint32_t *d_out_node,
                                       uint32_t *d_out_count, dann_query_stats *d_out_stats, cudaStream_t st) {
     const IndexView &v = ix->v;
-    if (B <= 0 || k <= 0) return fail(DANN_ERR_INVALID_ARG, "B and k must be positive");
-    if (L < 1 || L > 10000) return fail(DANN_ERR_INVALID_ARG, "search_list_size %d outside 1..10000 (guc.rs:11-26)", L);
-    if (rescore < 0 || rescore > 1000) return fail(DANN_ERR_INVALID_ARG, "rescore %d outside 0..1000 (guc.rs:28-43)", rescore);
     if (!d_queries || !d_out_tid) return fail(DANN_ERR_INVALID_ARG, "NULL query or output buffer");
-    if (ix->plain) {
-        if (d_label_off) return fail(DANN_ERR_INVALID_ARG, "plain storage does not support label filters (plain/storage.rs:260)");
-        /* scan.rs:392-403: a plain index only resorts when it holds fewer dimensions than the heap column */
-        if (v.dim == v.dim_index) rescore = 0;
-    }
-    if (rescore > 0 && v.n && !v.vectors) return fail(DANN_ERR_STATE, "index has no heap vectors yet (dann_index_set_vectors): rescore must be 0");
-    /* rows needed from the approximate stream: scan.rs:255-305 */
-    const uint32_t c_target = rescore == 0 ? (uint32_t)k : (uint32_t)rescore + (uint32_t)k - 1u;
-    /* the rerank kernel keeps the query row, one f32 per streamed row and the window in shared memory; a request past
-     * the limit is refused here, because a failed launch would poison the handle */
-    const size_t rerank_smem = rerank_smem_bytes(v.dim, c_target, (uint32_t)rescore);
-    if (rerank_smem > ix->rerank_smem_max)
-        return fail(DANN_ERR_INVALID_ARG, "k=%d rows with rescore=%d need %zu B of shared memory per scan (limit %zu): "
-                    "fetch fewer rows per scan", k, rescore, rerank_smem, ix->rerank_smem_max);
+    if (!bp.keyed) d_labels = nullptr, d_label_off = nullptr;
+    const uint32_t c_target = bp.c_target;
 
     CK(ix->sc_qfull.reserve((size_t)B * v.dim * sizeof(float)));
     CK(ix->sc_qcodes.reserve((size_t)B * v.cw * sizeof(uint64_t)));
@@ -868,6 +954,12 @@ static int search_batch_device_locked(dann_index *ix, const float *d_queries, co
     CK(ix->sc_stats.reserve((size_t)B * sizeof(dann_query_stats)));
     CK(ix->sc_qlist.reserve((size_t)B * sizeof(uint32_t)));
     CK(ix->sc_ctl.reserve(64));
+    const QueryParam *d_qp = nullptr;
+    if (!bp.qp.empty()) { /* ordered on st behind the queries and keys the caller staged */
+        CK(ix->sc_qparams.reserve(bp.qp.size() * sizeof(QueryParam)));
+        CK(cudaMemcpyAsync(ix->sc_qparams.p, bp.qp.data(), bp.qp.size() * sizeof(QueryParam), cudaMemcpyHostToDevice, st));
+        d_qp = ix->sc_qparams.as<QueryParam>();
+    }
     dann_query_stats *d_stats = d_out_stats ? d_out_stats : ix->sc_stats.as<dann_query_stats>();
 
     ix->timing = dann_batch_timing{};
@@ -878,8 +970,8 @@ static int search_batch_device_locked(dann_index *ix, const float *d_queries, co
     if (rc) return rc;
     CK(cudaEventRecord(ix->ev[1], st));
 
-    rc = run_search(ix, ix->sc_qcodes.as<uint64_t>(), d_labels, d_label_off, B, (uint32_t)L, c_target, d_stats, nullptr,
-                    nullptr, 0, st, ix->sc_qindex.as<float>());
+    rc = run_search(ix, ix->sc_qcodes.as<uint64_t>(), d_labels, d_label_off, B, (uint32_t)bp.L, c_target, d_stats, nullptr,
+                    nullptr, 0, st, ix->sc_qindex.as<float>(), d_qp);
     if (rc) return rc;
     CK(cudaEventRecord(ix->ev[2], st));
 
@@ -889,19 +981,20 @@ static int search_batch_device_locked(dann_index *ix, const float *d_queries, co
     r.stream = ix->sc_stream.as<uint32_t>();
     r.stream_len = ix->sc_stream_len.as<uint32_t>();
     r.c_target = c_target;
-    r.k = (uint32_t)k;
-    r.rescore = (uint32_t)rescore;
+    r.k = (uint32_t)bp.k;
+    r.rescore = (uint32_t)bp.rescore;
     r.out_tid = d_out_tid;
     r.out_dist = d_out_dist;
     r.out_node = d_out_node;
     r.out_count = d_out_count;
     r.stats = d_stats;
-    CK(allow_dynamic_smem(dann_rerank_kernel, rerank_smem));
-    dann_rerank_kernel<<<B, 128, rerank_smem, st>>>(r);
+    r.qp = d_qp;
+    CK(allow_dynamic_smem(dann_rerank_kernel, bp.rerank_smem));
+    dann_rerank_kernel<<<B, 128, bp.rerank_smem, st>>>(r);
     ix->launches++;
     CK(cudaGetLastError());
-    if (ix->plain && rescore > 0) {
-        dann_plain_stats_kernel<<<(B + 127) / 128, 128, 0, st>>>(d_stats, B);
+    if (ix->plain && bp.rescore > 0) {
+        dann_plain_stats_kernel<<<(B + 127) / 128, 128, 0, st>>>(d_stats, B, d_qp);
         ix->launches++;
         CK(cudaGetLastError());
     }
@@ -926,20 +1019,49 @@ extern "C" int dann_search_batch_device(dann_index *ix, const float *d_queries, 
                                         uint32_t *d_out_count, dann_query_stats *d_out_stats, void *stream) try {
     int rc = check_live(ix);
     if (rc) return rc;
+    BatchParams bp;
+    rc = uniform_params(ix, B, k, search_list_size, rescore, d_label_off != nullptr, &bp);
+    if (rc) return rc;
     std::lock_guard<std::mutex> lk(ix->mu);
     DANN_DEVICE_INPUT_STREAM(st, stream);
-    return search_batch_device_locked(ix, d_queries, d_labels, d_label_off, B, k, search_list_size, rescore,
-                                      d_out_tid, d_out_dist, nullptr, d_out_count, d_out_stats, st);
+    return search_batch_device_locked(ix, d_queries, d_labels, d_label_off, B, bp, d_out_tid, d_out_dist, nullptr,
+                                      d_out_count, d_out_stats, st);
+} DANN_CATCH
+
+extern "C" int dann_search_batch_mixed_device(dann_index *ix, const float *d_queries, const int16_t *d_labels,
+                                              const int32_t *d_label_off, const dann_query_params *d_params, int B,
+                                              uint64_t *d_out_tid, float *d_out_dist, uint32_t *d_out_count,
+                                              dann_query_stats *d_out_stats, void *stream) try {
+    int rc = check_live(ix);
+    if (rc) return rc;
+    if (B <= 0) return fail(DANN_ERR_INVALID_ARG, "B %d must be positive", B);
+    if (!d_params) return fail(DANN_ERR_INVALID_ARG, "params is NULL");
+    std::lock_guard<std::mutex> lk(ix->mu);
+    DANN_DEVICE_INPUT_STREAM(st, stream);
+    /* the checks read params and label_off on the host: one small read-back each, before anything runs */
+    std::vector<dann_query_params> hp((size_t)B);
+    std::vector<int32_t> hoff;
+    CK(cudaMemcpyAsync(hp.data(), d_params, (size_t)B * sizeof(dann_query_params), cudaMemcpyDeviceToHost, st));
+    if (d_label_off) {
+        hoff.resize((size_t)B + 1);
+        CK(cudaMemcpyAsync(hoff.data(), d_label_off, ((size_t)B + 1) * sizeof(int32_t), cudaMemcpyDeviceToHost, st));
+    }
+    CK(cudaStreamSynchronize(st));
+    BatchParams bp;
+    rc = mixed_params(ix, B, hp.data(), d_labels, d_label_off ? hoff.data() : nullptr, 0, &bp);
+    if (rc) return rc;
+    return search_batch_device_locked(ix, d_queries, d_labels, d_label_off, B, bp, d_out_tid, d_out_dist, nullptr,
+                                      d_out_count, d_out_stats, st);
 } DANN_CATCH
 
 /* The device half of the host-buffer batch: stages B host queries (and label keys) on ix's device and runs the batch
  * there.  Returns with the rows in ix->st_tid / st_dist / sc_node / st_count / st_stats and ix->stream drained.  The
  * caller holds ix->mu. */
 static int search_batch_staged_locked(dann_index *ix, const float *queries, const int16_t *labels,
-                                      const int32_t *label_off, int B, int k, int L, int rescore) {
+                                      const int32_t *label_off, int B, const BatchParams &bp) {
     cudaStream_t st = ix->stream;
     const IndexView &v = ix->v;
-    const size_t nk = (size_t)B * k;
+    const size_t nk = (size_t)B * bp.k;
     CK(ix->st_queries.reserve((size_t)B * v.dim * sizeof(float)));
     CK(ix->st_tid.reserve(nk * sizeof(uint64_t)));
     CK(ix->st_dist.reserve(nk * sizeof(float)));
@@ -951,7 +1073,7 @@ static int search_batch_staged_locked(dann_index *ix, const float *queries, cons
     const int32_t *d_off = nullptr;
     std::vector<int16_t> nl;
     std::vector<int32_t> no;
-    if (label_off) {
+    if (bp.keyed) {
         no.resize((size_t)B + 1);
         no[0] = 0;
         if (label_off[0] < 0) return fail(DANN_ERR_INVALID_ARG, "label_off[0] is negative");
@@ -969,23 +1091,28 @@ static int search_batch_staged_locked(dann_index *ix, const float *queries, cons
         d_lab = ix->st_labels.as<int16_t>();
         d_off = ix->st_label_off.as<int32_t>();
     }
-    return search_batch_device_locked(ix, ix->st_queries.as<float>(), d_lab, d_off, B, k, L, rescore,
-                                      ix->st_tid.as<uint64_t>(), ix->st_dist.as<float>(), ix->sc_node.as<uint32_t>(),
-                                      ix->st_count.as<uint32_t>(), ix->st_stats.as<dann_query_stats>(), st);
+    return search_batch_device_locked(ix, ix->st_queries.as<float>(), d_lab, d_off, B, bp, ix->st_tid.as<uint64_t>(),
+                                      ix->st_dist.as<float>(), ix->sc_node.as<uint32_t>(), ix->st_count.as<uint32_t>(),
+                                      ix->st_stats.as<dann_query_stats>(), st);
 }
 
-/* host-buffer batch with optional node ids (used by the scan operator too) */
-static int search_batch_host(dann_index *ix, const float *queries, const int16_t *labels,
-                             const int32_t *label_off, int B, int k, int L, int rescore, uint64_t *out_tid,
-                             float *out_dist, uint32_t *out_node, uint32_t *out_count,
-                             dann_query_stats *out_stats) {
-    int rc = check_live(ix);
-    if (rc) return rc;
-    if (B <= 0 || k <= 0 || !queries || !out_tid) return fail(DANN_ERR_INVALID_ARG, "dann_search_batch: bad argument");
+/* the uniform batch of a caller that holds ix->mu (dann_shards) */
+static int search_batch_staged_locked(dann_index *ix, const float *queries, const int16_t *labels,
+                                      const int32_t *label_off, int B, int k, int L, int rescore) {
+    BatchParams bp;
+    const int rc = uniform_params(ix, B, k, L, rescore, label_off != nullptr, &bp);
+    return rc ? rc : search_batch_staged_locked(ix, queries, labels, label_off, B, bp);
+}
+
+/* host-buffer batch with optional node ids; bp from uniform_params or mixed_params (rows of bp.k) */
+static int search_batch_host(dann_index *ix, const float *queries, const int16_t *labels, const int32_t *label_off, int B,
+                             const BatchParams &bp, uint64_t *out_tid, float *out_dist, uint32_t *out_node,
+                             uint32_t *out_count, dann_query_stats *out_stats) {
+    if (!queries || !out_tid) return fail(DANN_ERR_INVALID_ARG, "dann_search_batch: bad argument");
     std::lock_guard<std::mutex> lk(ix->mu);
     cudaStream_t st = ix->stream;
-    const size_t nk = (size_t)B * k;
-    rc = search_batch_staged_locked(ix, queries, labels, label_off, B, k, L, rescore);
+    const size_t nk = (size_t)B * bp.k;
+    int rc = search_batch_staged_locked(ix, queries, labels, label_off, B, bp);
     if (rc) return rc;
     CK(cudaMemcpyAsync(out_tid, ix->st_tid.p, nk * sizeof(uint64_t), cudaMemcpyDeviceToHost, st));
     if (out_dist) CK(cudaMemcpyAsync(out_dist, ix->st_dist.p, nk * sizeof(float), cudaMemcpyDeviceToHost, st));
@@ -996,12 +1123,36 @@ static int search_batch_host(dann_index *ix, const float *queries, const int16_t
     return DANN_OK;
 }
 
+static int search_batch_host(dann_index *ix, const float *queries, const int16_t *labels,
+                             const int32_t *label_off, int B, int k, int L, int rescore, uint64_t *out_tid,
+                             float *out_dist, uint32_t *out_node, uint32_t *out_count,
+                             dann_query_stats *out_stats) {
+    int rc = check_live(ix);
+    if (rc) return rc;
+    if (B <= 0 || k <= 0 || !queries || !out_tid) return fail(DANN_ERR_INVALID_ARG, "dann_search_batch: bad argument");
+    BatchParams bp;
+    rc = uniform_params(ix, B, k, L, rescore, label_off != nullptr, &bp);
+    if (rc) return rc;
+    return search_batch_host(ix, queries, labels, label_off, B, bp, out_tid, out_dist, out_node, out_count, out_stats);
+}
+
 extern "C" int dann_search_batch(dann_index *ix, const float *queries, const int16_t *labels,
                                  const int32_t *label_off, int B, int k, int search_list_size, int rescore,
                                  uint64_t *out_tid, float *out_dist, uint32_t *out_count,
                                  dann_query_stats *out_stats) try {
     return search_batch_host(ix, queries, labels, label_off, B, k, search_list_size, rescore, out_tid, out_dist,
                              nullptr, out_count, out_stats);
+} DANN_CATCH
+
+extern "C" int dann_search_batch_mixed(dann_index *ix, const float *queries, const int16_t *labels, const int32_t *label_off,
+                                       const dann_query_params *params, int B, uint64_t *out_tid, float *out_dist,
+                                       uint32_t *out_count, dann_query_stats *out_stats) try {
+    int rc = check_live(ix);
+    if (rc) return rc;
+    BatchParams bp;
+    rc = mixed_params(ix, B, params, labels, label_off, 0, &bp);
+    if (rc) return rc;
+    return search_batch_host(ix, queries, labels, label_off, B, bp, out_tid, out_dist, nullptr, out_count, out_stats);
 } DANN_CATCH
 
 /* ------------------------------------------------------------------------------------ */

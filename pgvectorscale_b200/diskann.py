@@ -71,6 +71,9 @@ class _ScanWorkspace(C.Structure):
                 ("device_bytes", C.c_uint64)]
 
 
+# dann_query_params, one per query of a mixed batch
+QUERY_PARAMS_DTYPE = np.dtype([("k", "<i4"), ("search_list_size", "<i4"), ("rescore", "<i4"), ("keyed", "<i4")])
+
 STATS_DTYPE = np.dtype([("visits", "<u4"), ("d_quantized", "<u4"), ("candidates", "<u4"),
                         ("d_full", "<u4"), ("stream_len", "<u4"), ("status", "<u4")])
 
@@ -80,6 +83,7 @@ EXPORTS = [
     "dann_coalescer_create", "dann_coalescer_search", "dann_coalescer_stats", "dann_coalescer_destroy",
     "dann_index_hbm_bytes", "dann_scan_begin", "dann_scan_rescan", "dann_scan_gettuple", "dann_scan_gettuple_many",
     "dann_coalescer_gettuple", "dann_scan_stats", "dann_scan_workspace", "dann_scan_end", "dann_search_batch", "dann_search_batch_device",
+    "dann_search_batch_mixed", "dann_search_batch_mixed_device", "dann_group_search_batch_mixed",
     "dann_prepare_queries", "dann_code_stride", "dann_sbq_distance", "dann_full_distance",
     "dann_kernel_launches", "dann_last_batch_timing",
     "dann_build_graph", "dann_index_download_nbrs", "dann_index_set_vectors", "dann_index_set_vectors_device",
@@ -130,6 +134,9 @@ def load_library(path: Optional[str] = None):
     lib.dann_search_batch.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp]
     lib.dann_search_batch_device.argtypes = [vp, vp, vp, vp, C.c_int, C.c_int, C.c_int, C.c_int,
                                              vp, vp, vp, vp, vp]
+    lib.dann_search_batch_mixed.argtypes = [vp, vp, vp, vp, vp, C.c_int, vp, vp, vp, vp]
+    lib.dann_search_batch_mixed_device.argtypes = [vp, vp, vp, vp, vp, C.c_int, vp, vp, vp, vp, vp]
+    lib.dann_group_search_batch_mixed.argtypes = [vp, vp, vp, vp, vp, C.c_int, vp, vp, vp, vp]
     lib.dann_prepare_queries.argtypes = [vp, vp, C.c_int, vp, vp, vp]
     lib.dann_sbq_distance.argtypes = [vp, vp, vp, vp, C.c_size_t, vp, vp]
     lib.dann_full_distance.argtypes = [vp, vp, vp, C.c_int, C.c_int, vp, vp]
@@ -333,7 +340,7 @@ class DiskAnnIndex:
 
     # -- batch ------------------------------------------------------------------------
     @staticmethod
-    def _labels_csr(labels: Optional[Sequence[Optional[Sequence[int]]]], B: int):
+    def _labels_csr(labels: Optional[Sequence[Optional[Sequence[int]]]], B: int, allow_unkeyed: bool = False):
         if labels is None:
             return None, None
         assert len(labels) == B
@@ -341,23 +348,46 @@ class DiskAnnIndex:
         vals = []
         for i, ls in enumerate(labels):
             if ls is None:
-                raise ValueError("a batch is either all unkeyed (labels=None) or all keyed")
-            vals.extend(int(x) for x in ls)
+                if not allow_unkeyed:
+                    raise ValueError("a batch is either all unkeyed (labels=None) or all keyed")
+            else:
+                vals.extend(int(x) for x in ls)
             off[i + 1] = len(vals)
         return np.asarray(vals, np.int16), off
 
-    def search_batch(self, queries, labels=None, k: int = 10,
-                     search_list_size: int = QUERY_SEARCH_LIST_SIZE_DEFAULT,
-                     rescore: int = QUERY_RESCORE_DEFAULT, out=None):
+    @staticmethod
+    def _batch_params(B: int, labels, k, search_list_size, rescore):
+        """None when every parameter is one int and no labels entry is None (the uniform dann_search_batch call), else
+        the QUERY_PARAMS_DTYPE array [B] of dann_search_batch_mixed."""
+        per_query = [np.ndim(x) > 0 for x in (k, search_list_size, rescore)]
+        unkeyed = labels is not None and any(ls is None for ls in labels)
+        if not any(per_query) and not unkeyed:
+            return None
+        p = np.empty(B, QUERY_PARAMS_DTYPE)
+        for name, x in (("k", k), ("search_list_size", search_list_size), ("rescore", rescore)):
+            a = np.asarray(x, dtype=np.int64)
+            if a.ndim > 0 and a.shape != (B,):
+                raise ValueError(f"{name} must be an int or a sequence of {B} ints")
+            p[name] = a
+        p["keyed"] = 0 if labels is None else [0 if ls is None else 1 for ls in labels]
+        return p
+
+    def search_batch(self, queries, labels=None, k=10, search_list_size=QUERY_SEARCH_LIST_SIZE_DEFAULT,
+                     rescore=QUERY_RESCORE_DEFAULT, out=None):
         """B independent index scans from host buffers; returns the first k rows of each.
 
-        queries: [B, dim] float32 (host).  labels: None, or one label list per query
-        (`labels && ARRAY[...]`).  Returns dict(tid[B,k] u64 = (block<<16)|offset with
-        INVALID_TID past count, dist[B,k] f32, count[B], stats[B])."""
+        queries: [B, dim] float32 (host).  labels: None, or one entry per query: a label list
+        (`labels && ARRAY[...]`) or None (no scan key).  k, search_list_size and rescore are each an int or a
+        sequence of B ints.  Returns dict(tid[B,kmax] u64 = (block<<16)|offset with INVALID_TID past count,
+        dist[B,kmax] f32, count[B], stats[B]), kmax = the largest k.  One int each and no None label entry is
+        dann_search_batch; anything else is dann_search_batch_mixed, with the same rows per query."""
         q = np.ascontiguousarray(queries, dtype=np.float32)
         if q.ndim != 2 or q.shape[1] != self.dim:
             raise ValueError(f"queries must be [B, {self.dim}]")
         B = q.shape[0]
+        params = self._batch_params(B, labels, k, search_list_size, rescore)
+        if params is not None:
+            return self._search_batch_mixed(q, labels, params, out)
         lab, off = self._labels_csr(labels, B)
         if out is None:
             out = dict(tid=np.empty((B, k), np.uint64), dist=np.empty((B, k), np.float32),
@@ -367,6 +397,29 @@ class DiskAnnIndex:
             B, int(k), int(search_list_size), int(rescore),
             _np_ptr(out["tid"]), _np_ptr(out["dist"]), _np_ptr(out["count"]), _np_ptr(out["stats"])))
         return out
+
+    def _search_batch_mixed(self, q, labels, params, out):
+        B = q.shape[0]
+        lab, off = self._labels_csr(labels, B, allow_unkeyed=True)
+        kmax = int(params["k"].max()) if B else 0
+        if out is None:
+            out = dict(tid=np.empty((B, kmax), np.uint64), dist=np.empty((B, kmax), np.float32),
+                       count=np.empty(B, np.uint32), stats=np.empty(B, STATS_DTYPE))
+        _check(self._lib, self._lib.dann_search_batch_mixed(
+            self._h, _np_ptr(q), _np_ptr(lab) if lab is not None and lab.size else None, _np_ptr(off),
+            _np_ptr(params), B, _np_ptr(out["tid"]), _np_ptr(out["dist"]), _np_ptr(out["count"]),
+            _np_ptr(out["stats"])))
+        return out
+
+    def search_batch_mixed_device(self, d_queries, d_params, d_out_tid, d_out_dist=None, d_out_count=None,
+                                  d_out_stats=None, d_labels=None, d_label_off=None, stream: int = 0):
+        """dann_search_batch_mixed_device: every buffer in this device's HBM (torch CUDA tensors); d_params is
+        [B] QUERY_PARAMS_DTYPE records (an int32 tensor [B, 4]), outputs [B, kmax]."""
+        B = int(d_queries.shape[0])
+        _check(self._lib, self._lib.dann_search_batch_mixed_device(
+            self._h, _dev_ptr(d_queries), _dev_ptr(d_labels), _dev_ptr(d_label_off), _dev_ptr(d_params), B,
+            _dev_ptr(d_out_tid), _dev_ptr(d_out_dist), _dev_ptr(d_out_count), _dev_ptr(d_out_stats),
+            C.c_void_p(stream) if stream else None))
 
     def search_batch_ptrs(self, q_ptr: int, B: int, k: int, search_list_size: int, rescore: int,
                           tid_ptr: int, dist_ptr: int, count_ptr: int = 0, stats_ptr: int = 0,
@@ -511,10 +564,23 @@ class IndexGroup:
         self.size = int(self._lib.dann_group_size(h))
         del keep
 
-    def search_batch(self, queries, labels=None, k: int = 10, search_list_size: int = QUERY_SEARCH_LIST_SIZE_DEFAULT,
-                     rescore: int = QUERY_RESCORE_DEFAULT) -> dict:
+    def search_batch(self, queries, labels=None, k=10, search_list_size=QUERY_SEARCH_LIST_SIZE_DEFAULT,
+                     rescore=QUERY_RESCORE_DEFAULT) -> dict:
+        """As DiskAnnIndex.search_batch: k, search_list_size and rescore may be per-query sequences and labels
+        entries None (dann_group_search_batch_mixed)."""
         q = np.ascontiguousarray(queries, dtype=np.float32)
         B = q.shape[0]
+        params = DiskAnnIndex._batch_params(B, labels, k, search_list_size, rescore)
+        if params is not None:
+            lab, off = DiskAnnIndex._labels_csr(labels, B, allow_unkeyed=True)
+            kmax = int(params["k"].max()) if B else 0
+            out = dict(tid=np.empty((B, kmax), np.uint64), dist=np.empty((B, kmax), np.float32),
+                       count=np.empty(B, np.uint32), stats=np.empty(B, STATS_DTYPE))
+            _check(self._lib, self._lib.dann_group_search_batch_mixed(
+                self._h, _np_ptr(q), _np_ptr(lab) if lab is not None and lab.size else None, _np_ptr(off),
+                _np_ptr(params), B, _np_ptr(out["tid"]), _np_ptr(out["dist"]), _np_ptr(out["count"]),
+                _np_ptr(out["stats"])))
+            return out
         lab, off = DiskAnnIndex._labels_csr(labels, B)
         out = dict(tid=np.empty((B, k), np.uint64), dist=np.empty((B, k), np.float32),
                    count=np.empty(B, np.uint32), stats=np.empty(B, STATS_DTYPE))
