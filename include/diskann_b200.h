@@ -13,7 +13,7 @@
  *     TSVScanState::initialize      scan.rs:57-88
  *     LabeledVector::from_scan_key_data labels/mod.rs:209-238
  *     Graph::greedy_search_streaming_init graph/mod.rs:331-354
- *   amgettuple             scan.rs:370-436           dann_scan_gettuple
+ *   amgettuple             scan.rs:370-436           dann_scan_gettuple (dann_scan_fetch: n calls' rows in one step)
  *     TSVResponseIterator::next_with_resort scan.rs:244-305
  *     Graph::greedy_search_iterate  graph/mod.rs:357-385
  *     SbqSpeedupStorage::visit_lsn  sbq/storage.rs:125-190
@@ -127,7 +127,8 @@ int dann_scan_rescan(dann_scan *sc, const float *query, const int16_t *labels, i
                      int search_list_size, int rescore);
 /* How far a scan may stream: to the end of the index, as the reference's next_with_resort does, with exactly its rows,
  * dist bits and dann_scan_stats after every call.  The only condition is device memory for the search state: a
- * failed allocation returns DANN_ERR_OOM.  The suspended search's workspace is planned for rescore + 64 streamed rows;
+ * failed allocation returns DANN_ERR_OOM.  The suspended search's workspace is planned for rescore + 64 streamed rows
+ * (for more when the first dann_scan_fetch after the rescan asks for more);
  * a scan that runs past it (a selective post-filter, or no LIMIT) has its workspace rebuilt twice as large and the
  * stream replayed from row 0 - invisible to the caller except in time.  Where that planned workspace can grow no
  * further (eight doublings in one call, or a visited list past shared memory, or 2^30 candidates) the scan enters the
@@ -142,6 +143,21 @@ int dann_scan_rescan(dann_scan *sc, const float *query, const int16_t *labels, i
  * dist is the exact rerank distance (NaN when rescore == 0). Any output may be NULL. */
 int dann_scan_gettuple(dann_scan *sc, uint32_t *block, uint16_t *offset, uint32_t *node_id,
                        float *dist);
+/* The next rows of a scan in one GPU step: exactly what max_rows consecutive dann_scan_gettuple calls return.
+ * Returns r = rows produced (0..max_rows; r < max_rows only at end of scan) or < 0.  block/offset/node_id/dist are
+ * [max_rows] (each may be NULL); row_stats[i] (may be NULL) = dann_scan_stats after the (i+1)-th of those calls.
+ * Afterwards the scan is in the state those max_rows calls leave: dann_scan_stats == row_stats[r-1] when r == max_rows,
+ * and when r < max_rows the counters of the call that found the end of scan (its search may have run on past the last
+ * row).  The next dann_scan_gettuple / dann_scan_fetch / dann_scan_gettuple_many continues the same stream, and the
+ * three may be interleaved at any call.  Rows, dist bits and counters never differ from the single calls'; the one
+ * thing that may is dann_scan_workspace: the eight replay regrows before the deep mode are counted per call, so a fetch
+ * may enter the deep mode at a different row than single calls would.  The search, the exact distances and the window
+ * step run once for all the rows (a fixed number of kernel launches, whatever max_rows), and the rows come back in one
+ * copy and one synchronisation; growing the workspace adds attempts, as in dann_scan_gettuple.
+ * Arguments are checked as dann_scan_gettuple checks them; in addition max_rows outside 1..65536 returns
+ * DANN_ERR_INVALID_ARG before anything runs.  A failed fetch fails as a failed dann_scan_gettuple does. */
+int dann_scan_fetch(dann_scan *sc, int max_rows, uint32_t *block, uint16_t *offset, uint32_t *node_id,
+                    float *dist, dann_query_stats *row_stats);
 /* n amgettuple calls, one per scan, all on the same index: out_rc[i] = 1 (row), 0 (end of scan) or a negative status
  * for that scan alone; block/offset/node_id/dist are [n] arrays, each may be NULL.
  * Every scan gets exactly the row, dist bits and dann_scan_stats the same sequence of dann_scan_gettuple calls would

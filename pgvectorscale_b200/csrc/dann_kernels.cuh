@@ -3,7 +3,7 @@
 //   sbq_distance     : stand-alone batched SBQ XOR+popcount gather (the roofline kernel)
 //   full_distance    : exact f32 L2 / cosine / inner product, AVX2 summation order
 //   rerank           : get_full_distance_for_resort + the sliding rerank window, a batch at a time
-//   scan_distance / scan_finish : the same for the streaming scan, one amgettuple at a time
+//   scan_distance / scan_finish : the same for the streaming scan, the rows of one or more amgettuple calls per step
 //   scan_distance_many / scan_finish_many : one amgettuple of each of many scans per launch
 //   normalize_rows / pad_rows / check_unique : index load helpers
 // Reference paths are relative to pgvectorscale/src/access_method/.
@@ -444,47 +444,55 @@ __global__ void dann_check_unique_kernel(const uint32_t *nbrs, uint32_t n, uint3
 }
 
 /* ------------------------------------------------------------------------------------ */
-/* Streaming scan (dann_scan_gettuple): one step of next_with_resort (scan.rs:244-305) per amgettuple, with one host
- * synchronisation.  The search launch, dann_scan_distance_kernel (exact distances of the rows the search appended) and
- * dann_scan_finish_kernel (the window step) are enqueued back to back; the two kernels read the search's outcome (rows
- * produced, overflow bits) from device memory, and the last one gathers everything the host needs into one ScanStepOut.
- * A search that overflowed its workspace leaves the window alone.  The rerank window lives in HBM between calls: win[]
- * is the BinaryHeap<ResortData> array, entries (total_cmp key of the exact distance << 32) | node. */
+/* Streaming scan (dann_scan_gettuple, dann_scan_fetch): one step of next_with_resort (scan.rs:244-305) yields the rows of
+ * one or more consecutive amgettuple calls, with one host synchronisation.  The search launch, dann_scan_distance_kernel
+ * (exact distances of the rows the search appended) and dann_scan_finish_kernel (the window step) are enqueued back to
+ * back; the two kernels read the search's outcome (rows produced, overflow bits) from device memory, and the last one
+ * gathers everything the host needs into one ScanStepOut and one ScanRow per row.  A search that overflowed its
+ * workspace leaves the window alone.  The rerank window lives in HBM between calls: win[] is the
+ * BinaryHeap<ResortData> array, entries (total_cmp key of the exact distance << 32) | node. */
 struct ScanWindow {
     uint32_t len, d_full;
 };
+/* one row of a step, with the scan's counters after the amgettuple call that would have returned it */
 struct ScanRow {
     uint64_t tid;
-    uint32_t node, have;
+    uint32_t node;
     float dist;
-    uint32_t pad;
+    uint32_t end;                /* the stream index its refill ended at */
+    uint32_t d_full;             /* the window's full-distance comparisons after its refill */
+    uint32_t visits, candidates; /* the search's counters */
 };
 struct ScanStepOut {
     uint32_t overflow, slen;
-    dann_query_stats stats;
-    ScanRow row;
+    uint32_t nrows, pad;     /* rows produced: fewer than asked only at end of scan */
+    dann_query_stats stats;  /* the search's counters at the end of the step */
     ScanWindow win;
 };
+#define DANN_SCAN_WIN_MAX 1000u /* the largest window: rescore <= 1000 */
 
-/* Exact distances of the rows a scan's search appended past `skip` (none when it overflowed), into out[skip, slen).
+/* Exact distances of the rows a scan's search appended in [begin, begin + span) (none when it overflowed), into out[].
  * qs: the dynamic window, [dim rounded up to 4].  Block-wide. */
 __device__ __forceinline__ void scan_distance_step(const IndexView &ix, float *qs, uint64_t *bar, const float *q_full,
                                                    const uint32_t *stream, const uint32_t *slen_p,
-                                                   const uint32_t *overflow_p, uint32_t skip, float *out) {
+                                                   const uint32_t *overflow_p, uint32_t begin, uint32_t span, float *out) {
     if (*overflow_p) return;
     const uint32_t slen = *slen_p;
-    if (slen <= skip) return;
+    if (slen <= begin) return;
+    const uint32_t end = slen - begin > span ? begin + span : slen;
     stage_query_row(qs, q_full, ix.dim, bar);
-    full_distances(ix, qs, stream, skip, slen, out);
+    full_distances(ix, qs, stream, begin, end, out);
 }
 
+/* CTA b: rows [skip + b * span, skip + (b + 1) * span) of the step; the host sizes the grid from the rows the search
+ * may append, and CTAs past the rows it did append exit */
 __global__ void __launch_bounds__(128) dann_scan_distance_kernel(IndexView ix, const float *q_full, const uint32_t *stream,
                                                                  const uint32_t *slen_p, const uint32_t *overflow_p,
-                                                                 uint32_t skip, float *out) {
+                                                                 uint32_t skip, uint32_t span, float *out) {
     DANN_DYN_SMEM(dann_smem);
     float *qs = reinterpret_cast<float *>(dann_smem);
     DANN_STATIC_SMEM uint64_t bar;
-    scan_distance_step(ix, qs, &bar, q_full, stream, slen_p, overflow_p, skip, out);
+    scan_distance_step(ix, qs, &bar, q_full, stream, slen_p, overflow_p, skip + blockIdx.x * span, span, out);
 }
 
 /* One amgettuple step of many scans (dann_scan_gettuple_many, and the first step of a sharded scan): the arguments
@@ -513,76 +521,114 @@ __global__ void __launch_bounds__(128) dann_scan_distance_many_kernel(const Inde
     float *qs = reinterpret_cast<float *>(dann_smem);
     DANN_STATIC_SMEM uint64_t bar;
     const ScanDistanceDesc &e = d[blockIdx.x];
-    scan_distance_step(views[e.view], qs, &bar, e.q_full, e.stream, e.slen_p, e.overflow_p, e.skip, e.out);
+    scan_distance_step(views[e.view], qs, &bar, e.q_full, e.stream, e.slen_p, e.overflow_p, e.skip, 0xFFFFFFFFu, e.out);
 }
 
-/* The window step of one scan: next_with_resort's refill with the rows its search appended, then one pop; *out gathers
- * what the host needs (overflow bits, rows produced, counters, the row, the window) */
-__device__ __forceinline__ void scan_finish_step(const IndexView &ix, ScanWindow *w, uint64_t *win, uint32_t rescore,
-                                                 const uint32_t *stream, const float *dist, uint32_t skip,
-                                                 const uint32_t *slen_p, uint32_t slen_fixed, const uint32_t *overflow_p,
-                                                 const dann_query_stats *stats_p, ScanStepOut *out) {
+/* The window step of one scan, on one thread: for each of up to nrows rows, next_with_resort's refill (push stream rows
+ * until the window holds `rescore`, or the rows the search appended run out), then one pop; with rescore == 0 the rows
+ * in stream order.  rows[r] gets row r's node, distance, refill end and d_full (scan_row_fill adds its tid and
+ * counters); *out gathers the step (overflow bits, rows appended and produced, final counters, the window).  win is the
+ * window's heap array: in HBM, or a shared-memory copy of it. */
+__device__ __forceinline__ void scan_finish_step(ScanWindow *w, uint64_t *win, uint32_t rescore, const uint32_t *stream,
+                                                 const float *dist, uint32_t skip, const uint32_t *slen_p, uint32_t slen_fixed,
+                                                 const uint32_t *overflow_p, const dann_query_stats *stats_p, uint32_t nrows,
+                                                 ScanStepOut *out, ScanRow *rows) {
     ScanStepOut o;
     o.overflow = overflow_p ? *overflow_p : 0u;
     o.slen = slen_p ? *slen_p : slen_fixed; /* no search this call: nothing new beyond `skip` */
+    o.nrows = 0;
+    o.pad = 0;
     o.stats = *stats_p;
-    o.row.tid = DANN_INVALID_TID;
-    o.row.node = DANN_INVALID_NODE;
-    o.row.have = 0;
-    o.row.dist = DANN_NAN_F;
-    o.row.pad = 0;
+    o.win = *w;
     if (o.overflow) { /* the host regrows the workspace and replays: the window must not move */
-        o.win = *w;
         *out = o;
         return;
     }
-    const uint32_t nnew = o.slen;
+    uint32_t pos = skip;
     if (rescore == 0) { /* resort_buffer.capacity() == 0: the stream order is the result (scan.rs:251-253) */
-        if (nnew > skip) {
-            o.row.node = stream[skip];
-            o.row.tid = ix.tids[o.row.node];
-            o.row.have = 1;
+        for (; o.nrows < nrows && pos < o.slen; o.nrows++, pos++) {
+            ScanRow &x = rows[o.nrows];
+            x.node = stream[pos];
+            x.dist = DANN_NAN_F;
+            x.end = pos + 1;
+            x.d_full = o.win.d_full;
         }
-        o.win = *w;
         *out = o;
         return;
     }
     using H = RustHeap<uint64_t, 32>;
     ArrayStore<uint64_t> store{win};
-    uint32_t len = w->len, dfull = w->d_full;
-    for (uint32_t i = skip; i < nnew; i++) { /* full_distance_comparisons += 1; resort_buffer.push(..) */
-        H::push(store, len, ((uint64_t)total_ukey(dist[i]) << 32) | stream[i]);
-        dfull++;
+    uint32_t len = o.win.len, dfull = o.win.d_full;
+    for (; o.nrows < nrows; o.nrows++) {
+        for (; len < rescore && pos < o.slen; pos++) { /* full_distance_comparisons += 1; resort_buffer.push(..) */
+            H::push(store, len, ((uint64_t)total_ukey(dist[pos]) << 32) | stream[pos]);
+            dfull++;
+        }
+        if (len == 0) break;
+        const uint64_t e = H::pop(store, len);
+        ScanRow &x = rows[o.nrows];
+        x.node = (uint32_t)e;
+        x.dist = total_ukey_inverse((uint32_t)(e >> 32));
+        x.end = pos;
+        x.d_full = dfull;
     }
-    if (len > 0) {
-        uint64_t e = H::pop(store, len);
-        o.row.node = (uint32_t)e;
-        o.row.dist = total_ukey_inverse((uint32_t)(e >> 32));
-        o.row.tid = ix.tids[o.row.node];
-        o.row.have = 1;
-    }
-    w->len = len;
-    w->d_full = dfull;
-    o.win.len = len;
-    o.win.d_full = dfull;
+    w->len = o.win.len = len;
+    w->d_full = o.win.d_full = dfull;
     *out = o;
 }
 
-__global__ void dann_scan_finish_kernel(IndexView ix, ScanWindow *w, uint64_t *win, uint32_t rescore, const uint32_t *stream,
-                                        const float *dist, uint32_t skip, const uint32_t *slen_p, uint32_t slen_fixed,
-                                        const uint32_t *overflow_p, const dann_query_stats *stats_p, ScanStepOut *out) {
-    if (threadIdx.x != 0 || blockIdx.x != 0) return;
-    scan_finish_step(ix, w, win, rescore, stream, dist, skip, slen_p, slen_fixed, overflow_p, stats_p, out);
+/* Row r's tid and counters.  Its refill asked for the stream up to index skip + first + r (first = the rows the step's
+ * first refill asked for).  If it got them all, the call that returns it would have stopped its search right after
+ * appending the last of them: the counters at that row (snap; a one-row step passes NULL, its search stopped there).
+ * If the stream ended during that refill or before it, or the step did not search, that call's search ran dry: the
+ * step's final counters st. */
+__device__ __forceinline__ void scan_row_fill(const IndexView &ix, ScanRow &x, uint32_t r, uint32_t first, uint32_t skip,
+                                              bool searched, const uint2 *snap, const dann_query_stats &st) {
+    x.tid = ix.tids[x.node];
+    if (searched && snap && x.end == skip + first + r) {
+        const uint2 c = snap[x.end - 1];
+        x.visits = c.x;
+        x.candidates = c.y;
+    } else {
+        x.visits = st.visits;
+        x.candidates = st.candidates;
+    }
 }
 
-/* thread i: the window step of scan d[i] on its index views[d[i].view], its outcome into out[i] (one copy brings every
- * scan's back) */
+/* One step of one scan (dann_scan_gettuple: nrows = 1; dann_scan_fetch): the window step on thread 0, then every row's
+ * tid and counters across the CTA.  A step of several rows stages the window (at most DANN_SCAN_WIN_MAX entries) in
+ * shared memory for its pushes and pops and writes it back once. */
+__global__ void __launch_bounds__(128) dann_scan_finish_kernel(IndexView ix, ScanWindow *w, uint64_t *win, uint32_t rescore,
+                                                               const uint32_t *stream, const float *dist, const uint2 *snap,
+                                                               uint32_t skip, const uint32_t *slen_p, uint32_t slen_fixed,
+                                                               const uint32_t *overflow_p, const dann_query_stats *stats_p,
+                                                               uint32_t nrows, ScanStepOut *out, ScanRow *rows) {
+    DANN_STATIC_SMEM uint64_t win_sm[DANN_SCAN_WIN_MAX];
+    const uint32_t len0 = w->len;
+    const bool stage = nrows > 1 && rescore > 0 && !(overflow_p && *overflow_p);
+    if (stage)
+        for (uint32_t i = threadIdx.x; i < len0; i += blockDim.x) win_sm[i] = win[i];
+    __syncthreads(); /* every thread has read the window before thread 0 moves it */
+    if (threadIdx.x == 0)
+        scan_finish_step(w, stage ? win_sm : win, rescore, stream, dist, skip, slen_p, slen_fixed, overflow_p, stats_p, nrows,
+                         out, rows);
+    __syncthreads();
+    const ScanStepOut &o = *out;
+    if (stage)
+        for (uint32_t i = threadIdx.x; i < o.win.len; i += blockDim.x) win[i] = win_sm[i];
+    const uint32_t first = rescore == 0 ? 1u : (len0 < rescore ? rescore - len0 : 0u);
+    for (uint32_t r = threadIdx.x; r < o.nrows; r += blockDim.x)
+        scan_row_fill(ix, rows[r], r, first, skip, slen_p != nullptr, snap, o.stats);
+}
+
+/* thread i: the one-row window step of scan d[i] on its index views[d[i].view], its outcome into out[i] and rows[i] (one
+ * copy brings every scan's back) */
 __global__ void __launch_bounds__(128) dann_scan_finish_many_kernel(const IndexView *views, const ScanFinishDesc *d,
-                                                                    uint32_t n, ScanStepOut *out) {
+                                                                    uint32_t n, ScanStepOut *out, ScanRow *rows) {
     const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const ScanFinishDesc f = d[i];
-    scan_finish_step(views[f.view], f.w, f.win, f.rescore, f.stream, f.dist, f.skip, f.slen_p, f.slen_fixed, f.overflow_p,
-                     f.stats_p, out + i);
+    scan_finish_step(f.w, f.win, f.rescore, f.stream, f.dist, f.skip, f.slen_p, f.slen_fixed, f.overflow_p, f.stats_p, 1u,
+                     out + i, rows + i);
+    if (out[i].nrows) scan_row_fill(views[f.view], rows[i], 0u, 1u, f.skip, f.slen_p != nullptr, nullptr, out[i].stats);
 }
-

@@ -421,7 +421,11 @@ struct SearchWarp {
             const uint32_t node = (uint32_t)e;
             const uint64_t tid = __ldg(ix.tids + node); /* return_lsn, sbq/storage.rs:404-414 */
             if ((tid & 0xFFFFull) == 0) continue;       /* InvalidOffsetNumber: deleted tuple, scan.rs:231-234 */
-            if (lane == 0) a.stream[(size_t)q * a.c_target + scount] = node;
+            if (lane == 0) {
+                a.stream[(size_t)q * a.c_target + scount] = node;
+                /* the counters a search that suspended right here would report (write_query_stats) */
+                if (a.row_counters) a.row_counters[(size_t)q * a.c_target + scount] = make_uint2(visits, dq);
+            }
             scount++;
             if (scount == query_c_target(a, q)) done = true;
         }

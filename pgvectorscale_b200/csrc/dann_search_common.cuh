@@ -70,6 +70,9 @@ struct SearchArgs {
     /* per-query L, c_target and key (indexed by query id, after the qlist mapping); NULL = L, c_target and q_label_off
      * above apply to every query.  The stream's row stride stays c_target, the batch maximum.  Kept last. */
     const QueryParam *qp = nullptr;
+    /* [B][c_target] (visits, dq) when stream row i was appended: what the query's counters would be had the search
+     * suspended right after that row (SearchWarp only, for a streaming scan's multi-row step); NULL = none.  Kept last. */
+    uint2 *row_counters = nullptr;
 };
 #define DANN_HV_POP 2u
 

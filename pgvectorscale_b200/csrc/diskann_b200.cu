@@ -198,7 +198,8 @@ struct dann_index {
     bool plain = false;
     const float *index_vectors = nullptr; /* [n][dim_index] in HBM */
     DevBuf sc_qindex;
-    /* dann_scan_gettuple_many: one round's per-scan launch arguments and descriptors, then its ScanStepOut array */
+    /* dann_scan_gettuple_many: one round's per-scan launch arguments and descriptors, then its ScanStepOut and ScanRow
+     * arrays */
     DevBuf sc_many;
 };
 
@@ -221,14 +222,17 @@ struct dann_scan {
     bool active = false;
     /* suspended search state in HBM (see SavedScan / dann_search_common.cuh) */
     DevBuf d_qindex; /* plain layout: the prepared index slice */
-    DevBuf d_step;   /* one ScanStepOut per amgettuple */
+    DevBuf d_step;   /* one step's ScanStepOut, then its ScanRow records */
+    DevBuf d_snap;   /* a multi-row step's counters at each stream row (SearchArgs::row_counters) */
     DevBuf d_query, d_qfull, d_qcodes, d_labels, d_label_off, d_saved, d_heap_sm, d_vis, d_heap_tail, d_cnode, d_set,
         d_ins, d_stream, d_slen, d_stats, d_dist, d_win, d_winst, d_ctl;
+    std::vector<unsigned char> h_step; /* the step's ScanStepOut and records, copied back */
     SearchPlan plan{};
     uint32_t grow = 1;
     bool deep = false;      /* plan is the deep plan (dann_make_deep_plan): the workspace grows in place */
     uint32_t regrows = 0;   /* replay regrows since the rescan */
     uint32_t growths = 0;   /* in-place growths since the rescan */
+    uint32_t plan_rows = 0; /* streamed rows the workspace is planned for (times grow): rescore + 64, or a first fetch's */
     uint32_t streamed = 0;  /* rows taken off the approximate stream so far */
     uint32_t win_len = 0;   /* rows sitting in the rerank window */
     bool exhausted = false; /* next() returned None */
@@ -1420,7 +1424,8 @@ extern "C" int dann_scan_begin(dann_index *ix, dann_scan **out) try {
 #define DANN_SCAN_BUFS(sc)                                                                                               \
     {&(sc)->d_qindex, &(sc)->d_step, &(sc)->d_query, &(sc)->d_qfull, &(sc)->d_qcodes, &(sc)->d_labels, &(sc)->d_label_off, \
      &(sc)->d_saved, &(sc)->d_heap_sm, &(sc)->d_vis, &(sc)->d_heap_tail, &(sc)->d_cnode, &(sc)->d_set, &(sc)->d_ins,       \
-     &(sc)->d_stream, &(sc)->d_slen, &(sc)->d_stats, &(sc)->d_dist, &(sc)->d_win, &(sc)->d_winst, &(sc)->d_ctl}
+     &(sc)->d_stream, &(sc)->d_slen, &(sc)->d_stats, &(sc)->d_dist, &(sc)->d_win, &(sc)->d_winst, &(sc)->d_ctl,     \
+     &(sc)->d_snap}
 
 static void scan_release(dann_scan *sc) {
     DevBuf *bufs[] = DANN_SCAN_BUFS(sc);
@@ -1431,7 +1436,7 @@ static void scan_release(dann_scan *sc) {
 static int scan_reset_search(dann_scan *sc, cudaStream_t st) {
     dann_index *ix = sc->ix;
     SearchPlan &p = sc->plan;
-    int rc = make_plan(ix, 1, (uint32_t)sc->L, (uint32_t)sc->rescore + 64u, sc->grow, sc->nlabels >= 0, &p, true);
+    int rc = make_plan(ix, 1, (uint32_t)sc->L, sc->plan_rows, sc->grow, sc->nlabels >= 0, &p, true);
     if (rc) return rc;
     CK(sc->d_saved.reserve(sizeof(SavedScan)));
     CK(sc->d_heap_sm.reserve((size_t)p.hs * p.esize + 16));
@@ -1479,9 +1484,10 @@ static int scan_rescan_enqueue(dann_scan *sc, const float *query, const int16_t 
     sc->L = search_list_size;
     sc->rescore = rescore;
     sc->grow = 1;
+    sc->plan_rows = (uint32_t)rescore + 64u;
     if (sc->deep) { /* back to the planned workspace: give the deep scan's buffers back (reserve() never shrinks) */
         DevBuf *deep_bufs[] = {&sc->d_heap_sm, &sc->d_vis, &sc->d_heap_tail, &sc->d_cnode, &sc->d_set, &sc->d_ins,
-                               &sc->d_stream, &sc->d_dist};
+                               &sc->d_stream, &sc->d_dist, &sc->d_snap};
         for (DevBuf *b : deep_bufs) b->release();
         sc->deep = false;
     }
@@ -1497,7 +1503,7 @@ static int scan_rescan_enqueue(dann_scan *sc, const float *query, const int16_t 
     CK(sc->d_stats.reserve(sizeof(dann_query_stats)));
     CK(sc->d_win.reserve((size_t)std::max(rescore, 1) * 8));
     CK(sc->d_winst.reserve(sizeof(ScanWindow)));
-    CK(sc->d_step.reserve(sizeof(ScanStepOut)));
+    CK(sc->d_step.reserve(sizeof(ScanStepOut) + sizeof(ScanRow)));
     CK(sc->d_ctl.reserve(64));
     CK(cudaMemcpyAsync(sc->d_query.p, sc->query.data(), (size_t)dim * 4, cudaMemcpyHostToDevice, st));
     if (sc->nlabels >= 0) {
@@ -1538,8 +1544,9 @@ extern "C" int dann_scan_rescan(dann_scan *sc, const float *query, const int16_t
 } DANN_CATCH
 
 /* The launch arguments of the scan's resumable search for rows [0, want) of this step: its plan, its private workspace
- * and its saved state (d_ctl[1] receives the overflow bits). */
-static int scan_search_args(dann_scan *sc, uint32_t want, SearchArgs *out) {
+ * and its saved state (d_ctl[1] receives the overflow bits).  counters: the step yields several rows, and the search
+ * records its counters at every row it appends (d_snap). */
+static int scan_search_args(dann_scan *sc, uint32_t want, bool counters, SearchArgs *out) {
     dann_index *ix = sc->ix;
     const IndexView &v = ix->v;
     {
@@ -1569,18 +1576,22 @@ static int scan_search_args(dann_scan *sc, uint32_t want, SearchArgs *out) {
         a.plain_vectors = ix->index_vectors;
         a.q_index = sc->d_qindex.as<float>();
         a.plain_dim = ix->plain ? v.dim_index : 0;
+        if (counters) {
+            CK(sc->d_snap.reserve((size_t)want * sizeof(uint2)));
+            a.row_counters = sc->d_snap.as<uint2>();
+        }
         *out = a;
     }
     return DANN_OK;
 }
 
 /* Enqueue the resumable search for rows [0, want) of this launch (d_ctl[1] receives the overflow bits). */
-static int scan_launch_search(dann_scan *sc, uint32_t want) {
+static int scan_launch_search(dann_scan *sc, uint32_t want, bool counters) {
     dann_index *ix = sc->ix;
     cudaStream_t st = ix->stream;
     const SearchPlan &p = sc->plan;
     SearchArgs a;
-    int rc = scan_search_args(sc, want, &a);
+    int rc = scan_search_args(sc, want, counters, &a);
     if (rc) return rc;
     CK(cudaMemsetAsync(sc->d_ctl.p, 0, 8, st));
     search_fn fn = pick_kernel(false, p.entry, ix->NCH, ix->plain, p.deep);
@@ -1591,11 +1602,11 @@ static int scan_launch_search(dann_scan *sc, uint32_t want) {
     return DANN_OK;
 }
 
-/* rows this amgettuple takes off the approximate stream: next_with_resort refills the window to `rescore`
- * (scan.rs:255-305), next() takes one */
-static uint32_t scan_step_need(const dann_scan *sc) {
+/* rows a step of nrows amgettuple calls takes off the approximate stream: next_with_resort refills the window to
+ * `rescore` (scan.rs:255-305) and each later call refills the one row its predecessor popped; next() takes one */
+static uint32_t scan_step_need(const dann_scan *sc, uint32_t nrows) {
     const uint32_t rescore = (uint32_t)sc->rescore;
-    return rescore == 0 ? 1u : (sc->win_len < rescore ? rescore - sc->win_len : 0u);
+    return rescore == 0 ? nrows : (sc->win_len < rescore ? rescore - sc->win_len : 0u) + nrows - 1;
 }
 
 /* dynamic shared memory of a scan-distance CTA: the query row */
@@ -1699,70 +1710,109 @@ static int scan_grow_in_place(dann_scan *sc, cudaStream_t st) {
     return DANN_OK;
 }
 
-/* The host side of a step that did not overflow: the stream position, end of stream and counters of the scan, then its
- * row.  `want` = rows [0, want) the search was asked for, the first `skip` of them replayed.  Returns 1 (row) or 0
- * (end of scan). */
-static int scan_after_step(dann_scan *sc, const ScanStepOut &o, bool searching, uint32_t want, uint32_t skip,
-                           uint32_t *block, uint16_t *offset, uint32_t *node_id, float *dist) {
-    if (searching) {
-        if (o.slen < want) sc->exhausted = true;
-        sc->streamed += o.slen > skip ? o.slen - skip : 0;
-        sc->stats = o.stats;
-    }
-    sc->win_len = o.win.len;
-    sc->stats.d_full = o.win.d_full;
-    if (sc->ix->plain) { /* every comparison of the beam search was a full-distance comparison (plain/storage.rs:238,288) */
-        sc->stats.d_full += sc->stats.candidates;
-        sc->stats.d_quantized = 0;
-    }
-    sc->stats.stream_len = sc->streamed;
-    if (!o.row.have) return 0;
-    if (block) *block = (uint32_t)(o.row.tid >> 16);
-    if (offset) *offset = (uint16_t)(o.row.tid & 0xFFFFu);
-    if (node_id) *node_id = o.row.node;
-    if (dist) *dist = o.row.dist;
-    return 1;
+/* The scan's counters after one amgettuple call: the search's (visits, candidates), the window's full-distance
+ * comparisons and the rows streamed so far */
+static void scan_set_counters(dann_scan *sc, uint32_t visits, uint32_t candidates, uint32_t d_full, uint32_t streamed) {
+    const bool plain = sc->ix->plain;
+    dann_query_stats &s = sc->stats;
+    s.visits = visits;
+    s.candidates = candidates;
+    s.d_quantized = plain ? 0u : candidates;
+    /* plain layout: every comparison of the beam search was a full-distance comparison (plain/storage.rs:238,288) */
+    s.d_full = d_full + (plain ? candidates : 0u);
+    s.stream_len = sc->streamed = streamed;
+    s.status = 0;
 }
 
-/* next_with_resort (scan.rs:244-305): `while resort_buffer.len() < resort_size { next() ... }` then pop; with
- * resort_size == 0 it is a plain next().  The search, the exact distances of the rows it appended and the window step
- * are enqueued back to back (see dann_scan_finish_kernel) and one ScanStepOut comes back: one host synchronisation. */
-extern "C" int dann_scan_gettuple(dann_scan *sc, uint32_t *block, uint16_t *offset, uint32_t *node_id, float *dist) try {
-    if (!sc) return fail(DANN_ERR_INVALID_ARG, "dann_scan_gettuple: NULL scan");
-    if (!sc->active) return fail(DANN_ERR_STATE, "dann_scan_gettuple before dann_scan_rescan");
+/* The host side of a step of nrows calls that did not overflow, applied row by row: each record's stream position,
+ * counters and row, then - when the step met the end of scan - the counters of the call that found it.  `want` = rows
+ * [0, want) the search was asked for, the first `skip` of them replayed.  row i goes to the outputs' element i.
+ * Returns the rows produced. */
+static int scan_after_step(dann_scan *sc, const ScanStepOut &o, const ScanRow *rows, uint32_t nrows, bool searching,
+                           uint32_t want, uint32_t skip, uint32_t *block, uint16_t *offset, uint32_t *node_id, float *dist,
+                           dann_query_stats *row_stats) {
+    const uint32_t streamed = sc->streamed;
+    if (searching && o.slen < want) sc->exhausted = true;
+    for (uint32_t r = 0; r < o.nrows; r++) {
+        const ScanRow &x = rows[r];
+        scan_set_counters(sc, x.visits, x.candidates, x.d_full, streamed + (x.end - skip));
+        if (row_stats) row_stats[r] = sc->stats;
+        if (block) block[r] = (uint32_t)(x.tid >> 16);
+        if (offset) offset[r] = (uint16_t)(x.tid & 0xFFFFu);
+        if (node_id) node_id[r] = x.node;
+        if (dist) dist[r] = x.dist;
+    }
+    if (o.nrows < nrows)
+        scan_set_counters(sc, o.stats.visits, o.stats.candidates, o.win.d_full, streamed + (o.slen > skip ? o.slen - skip : 0u));
+    sc->win_len = o.win.len;
+    return (int)o.nrows;
+}
+
+/* The next nrows rows of a scan in one step: exactly what nrows consecutive amgettuple calls return
+ * (next_with_resort, scan.rs:244-305: `while resort_buffer.len() < resort_size { next() ... }` then pop; with
+ * resort_size == 0 a plain next()).  The search, the exact distances of the rows it appended and the window step are
+ * enqueued back to back (see dann_scan_finish_kernel), and one ScanStepOut with the step's records comes back: one host
+ * synchronisation, more when the workspace must grow.  Returns the rows produced or < 0. */
+static int scan_fetch(dann_scan *sc, uint32_t nrows, const char *what, uint32_t *block, uint16_t *offset, uint32_t *node_id,
+                      float *dist, dann_query_stats *row_stats) {
+    if (!sc) return fail(DANN_ERR_INVALID_ARG, "%s: NULL scan", what);
+    if (!sc->active) return fail(DANN_ERR_STATE, "%s before dann_scan_rescan", what);
     dann_index *ix = sc->ix;
     int rc = check_live(ix);
     if (rc) return rc;
     std::lock_guard<std::mutex> lk(ix->mu);
     const IndexView &v = ix->v;
     cudaStream_t st = ix->stream;
-    const uint32_t need = scan_step_need(sc);
+    const uint32_t need = scan_step_need(sc, nrows);
     const bool searching = need && !sc->exhausted;
+    const size_t out_bytes = sizeof(ScanStepOut) + (size_t)nrows * sizeof(ScanRow);
+    CK(sc->d_step.reserve(out_bytes));
+    sc->h_step.resize(out_bytes);
+    if (searching && sc->streamed == 0 && !sc->deep && need > sc->plan_rows) {
+        /* the first step after amrescan asks for more rows than the workspace is planned for: plan for them before
+         * anything has streamed, instead of regrowing by replay; where no such plan exists, the planned workspace stays */
+        const SearchPlan last = sc->plan;
+        const uint32_t last_rows = sc->plan_rows;
+        sc->plan_rows = need;
+        rc = scan_reset_search(sc, st);
+        if (rc == DANN_ERR_CAPACITY) {
+            sc->plan = last;
+            sc->plan_rows = last_rows;
+        } else if (rc) {
+            return rc;
+        }
+    }
     ScanStepOut o;
     uint32_t skip = 0; /* rows that are only re-generated because the workspace had to grow */
     for (int attempt = 0;;) {
         const uint32_t want = skip + need;
         if (searching) {
-            rc = scan_launch_search(sc, want);
+            rc = scan_launch_search(sc, want, nrows > 1);
             if (rc) return rc;
             if (sc->rescore > 0) {
                 ScanDistanceDesc d;
                 rc = scan_distance_desc(sc, want, skip, &d);
                 if (rc) return rc;
+                const uint32_t span = 256; /* rows per CTA */
                 const size_t smem = scan_distance_smem(v);
                 CK(allow_dynamic_smem(dann_scan_distance_kernel, smem));
-                dann_scan_distance_kernel<<<1, 128, smem, st>>>(v, d.q_full, d.stream, d.slen_p, d.overflow_p, d.skip, d.out);
+                dann_scan_distance_kernel<<<(need + span - 1) / span, 128, smem, st>>>(v, d.q_full, d.stream, d.slen_p,
+                                                                                      d.overflow_p, d.skip, span, d.out);
                 ix->launches++;
                 CK(cudaGetLastError());
             }
         }
         const ScanFinishDesc f = scan_finish_desc(sc, searching, skip);
-        dann_scan_finish_kernel<<<1, 32, 0, st>>>(v, f.w, f.win, f.rescore, f.stream, f.dist, f.skip, f.slen_p, f.slen_fixed,
-                                                 f.overflow_p, f.stats_p, sc->d_step.as<ScanStepOut>());
+        ScanStepOut *d_out = sc->d_step.as<ScanStepOut>();
+        dann_scan_finish_kernel<<<1, 128, 0, st>>>(v, f.w, f.win, f.rescore, f.stream, f.dist,
+                                                   nrows > 1 ? sc->d_snap.as<uint2>() : nullptr, f.skip, f.slen_p,
+                                                   f.slen_fixed, f.overflow_p, f.stats_p, nrows, d_out,
+                                                   reinterpret_cast<ScanRow *>(d_out + 1));
         ix->launches++;
         CK(cudaGetLastError());
-        CK(cudaMemcpyAsync(&o, sc->d_step.p, sizeof o, cudaMemcpyDeviceToHost, st));
+        CK(cudaMemcpyAsync(sc->h_step.data(), d_out, out_bytes, cudaMemcpyDeviceToHost, st));
         CK(cudaStreamSynchronize(st));
+        memcpy(&o, sc->h_step.data(), sizeof o);
         if (!o.overflow) break;
         if (o.overflow == DANN_ST_GROW) { /* the same step resumes after the rows it already appended */
             rc = scan_grow_in_place(sc, st);
@@ -1773,19 +1823,32 @@ extern "C" int dann_scan_gettuple(dann_scan *sc, uint32_t *block, uint16_t *offs
         if (rc) return rc;
         skip = sc->streamed;
     }
-    return scan_after_step(sc, o, searching, skip + need, skip, block, offset, node_id, dist);
+    return scan_after_step(sc, o, reinterpret_cast<const ScanRow *>(sc->h_step.data() + sizeof(ScanStepOut)), nrows,
+                           searching, skip + need, skip, block, offset, node_id, dist, row_stats);
+}
+
+extern "C" int dann_scan_gettuple(dann_scan *sc, uint32_t *block, uint16_t *offset, uint32_t *node_id, float *dist) try {
+    return scan_fetch(sc, 1u, "dann_scan_gettuple", block, offset, node_id, dist, nullptr);
+} DANN_CATCH
+
+extern "C" int dann_scan_fetch(dann_scan *sc, int max_rows, uint32_t *block, uint16_t *offset, uint32_t *node_id,
+                               float *dist, dann_query_stats *row_stats) try {
+    if (max_rows < 1 || max_rows > 65536)
+        return fail(DANN_ERR_INVALID_ARG, "dann_scan_fetch: max_rows = %d outside 1..65536", max_rows);
+    return scan_fetch(sc, (uint32_t)max_rows, "dann_scan_fetch", block, offset, node_id, dist, row_stats);
 } DANN_CATCH
 
 /* The device part of one dann_scan_gettuple_many round: one upload of [IndexView x views][SearchArgs x args]
  * [ScanDistanceDesc x ddesc][ScanFinishDesc x fdesc], one dann_scan_search_many_kernel launch per run of equal fns[]
  * (args is grouped by instantiation), one dann_scan_distance_many_kernel launch when ddesc is not empty, one
- * dann_scan_finish_many_kernel launch, one download of the fdesc.size() outcomes into outs and one synchronisation.
+ * dann_scan_finish_many_kernel launch, one download of the fdesc.size() outcomes into outs and their rows into rows
+ * (through back), and one synchronisation.
  * The descriptors' `view` fields index views[]: the indexes of the round's scans, all on the device of `ix`, whose
  * stream, sc_many buffer and launch counter the round uses. */
 static int scan_many_round(dann_index *ix, const std::vector<IndexView> &views, const std::vector<scan_many_fn> &fns,
                            const std::vector<SearchArgs> &args, const std::vector<ScanDistanceDesc> &ddesc,
                            const std::vector<ScanFinishDesc> &fdesc, std::vector<unsigned char> &blob,
-                           std::vector<ScanStepOut> &outs) {
+                           std::vector<ScanStepOut> &outs, std::vector<ScanRow> &rows, std::vector<unsigned char> &back) {
     cudaStream_t st = ix->stream;
     const size_t m = fdesc.size();
     auto align16 = [](size_t b) { return (b + 15) & ~(size_t)15; };
@@ -1798,7 +1861,8 @@ static int scan_many_round(dann_index *ix, const std::vector<IndexView> &views, 
     if (!args.empty()) memcpy(blob.data() + o_args, args.data(), args.size() * sizeof(SearchArgs));
     if (!ddesc.empty()) memcpy(blob.data() + o_dist, ddesc.data(), ddesc.size() * sizeof(ScanDistanceDesc));
     memcpy(blob.data() + o_fin, fdesc.data(), m * sizeof(ScanFinishDesc));
-    CK(ix->sc_many.reserve(o_out + m * sizeof(ScanStepOut)));
+    const size_t o_rows = o_out + m * sizeof(ScanStepOut);
+    CK(ix->sc_many.reserve(o_rows + m * sizeof(ScanRow)));
     unsigned char *dev = ix->sc_many.as<unsigned char>();
     const IndexView *d_views = reinterpret_cast<const IndexView *>(dev);
     CK(cudaMemcpyAsync(dev, blob.data(), o_out, cudaMemcpyHostToDevice, st));
@@ -1824,12 +1888,17 @@ static int scan_many_round(dann_index *ix, const std::vector<IndexView> &views, 
         CK(cudaGetLastError());
     }
     dann_scan_finish_many_kernel<<<(unsigned)((m + 127) / 128), 128, 0, st>>>(
-        d_views, reinterpret_cast<const ScanFinishDesc *>(dev + o_fin), (uint32_t)m, reinterpret_cast<ScanStepOut *>(dev + o_out));
+        d_views, reinterpret_cast<const ScanFinishDesc *>(dev + o_fin), (uint32_t)m, reinterpret_cast<ScanStepOut *>(dev + o_out),
+        reinterpret_cast<ScanRow *>(dev + o_rows));
     ix->launches++;
     CK(cudaGetLastError());
     outs.resize(m);
-    CK(cudaMemcpyAsync(outs.data(), dev + o_out, m * sizeof(ScanStepOut), cudaMemcpyDeviceToHost, st));
+    rows.resize(m);
+    back.resize(m * (sizeof(ScanStepOut) + sizeof(ScanRow)));
+    CK(cudaMemcpyAsync(back.data(), dev + o_out, back.size(), cudaMemcpyDeviceToHost, st));
     CK(cudaStreamSynchronize(st));
+    memcpy(outs.data(), back.data(), m * sizeof(ScanStepOut));
+    memcpy(rows.data(), back.data() + m * sizeof(ScanStepOut), m * sizeof(ScanRow));
     return DANN_OK;
 }
 
@@ -1865,6 +1934,8 @@ static int scan_gettuple_many_locked(dann_index *lead, dann_scan *const *scans, 
     std::vector<ScanFinishDesc> fdesc;
     std::vector<unsigned char> blob;
     std::vector<ScanStepOut> outs;
+    std::vector<ScanRow> rows;
+    std::vector<unsigned char> back;
     searchers.reserve(n);
     live.reserve(n);
     next.reserve(n);
@@ -1873,6 +1944,8 @@ static int scan_gettuple_many_locked(dann_index *lead, dann_scan *const *scans, 
     ddesc.reserve(n);
     fdesc.reserve(n);
     outs.reserve(n);
+    rows.reserve(n);
+    back.reserve((size_t)n * (sizeof(ScanStepOut) + sizeof(ScanRow)));
     if (msgs) msgs->assign((size_t)n, std::string());
     for (int i = 0; i < n; i++) {
         dann_scan *sc = scans[i];
@@ -1881,7 +1954,7 @@ static int scan_gettuple_many_locked(dann_index *lead, dann_scan *const *scans, 
             indexes.push_back(sc->ix);
             views.push_back(sc->ix->v);
         }
-        const uint32_t need = scan_step_need(sc);
+        const uint32_t need = scan_step_need(sc, 1);
         steps[i] = Step{sc, i, need, 0u, need && !sc->exhausted, 0, nullptr, (uint32_t)view};
         round[i] = &steps[i];
     }
@@ -1914,7 +1987,7 @@ static int scan_gettuple_many_locked(dann_index *lead, dann_scan *const *scans, 
             const uint32_t want = s->skip + s->need;
             SearchArgs a;
             ScanDistanceDesc d{};
-            rc = scan_search_args(s->sc, want, &a);
+            rc = scan_search_args(s->sc, want, false, &a);
             if (!rc && s->sc->rescore > 0) rc = scan_distance_desc(s->sc, want, s->skip, &d);
             if (rc) { /* this scan's buffers: it leaves the round */
                 scan_failed(s, rc);
@@ -1935,7 +2008,7 @@ static int scan_gettuple_many_locked(dann_index *lead, dann_scan *const *scans, 
                 fdesc.back().view = s->view;
             }
         if (live.empty()) break;
-        rc = scan_many_round(lead, views, fns, args, ddesc, fdesc, blob, outs);
+        rc = scan_many_round(lead, views, fns, args, ddesc, fdesc, blob, outs, rows, back);
         if (rc) {
             if (!moved) return rc;
             for (Step *s : live) scan_failed(s, rc);
@@ -1946,8 +2019,9 @@ static int scan_gettuple_many_locked(dann_index *lead, dann_scan *const *scans, 
             Step *s = live[j];
             const int i = s->i;
             if (!outs[j].overflow) {
-                out_rc[i] = scan_after_step(s->sc, outs[j], s->searching, s->skip + s->need, s->skip, block ? block + i : nullptr,
-                                            offset ? offset + i : nullptr, node_id ? node_id + i : nullptr, dist ? dist + i : nullptr);
+                out_rc[i] = scan_after_step(s->sc, outs[j], &rows[j], 1u, s->searching, s->skip + s->need, s->skip,
+                                            block ? block + i : nullptr, offset ? offset + i : nullptr,
+                                            node_id ? node_id + i : nullptr, dist ? dist + i : nullptr, nullptr);
                 moved = true;
                 continue;
             }

@@ -83,6 +83,7 @@ EXPORTS = [
     "dann_coalescer_create", "dann_coalescer_search", "dann_coalescer_stats", "dann_coalescer_destroy",
     "dann_index_hbm_bytes", "dann_scan_begin", "dann_scan_rescan", "dann_scan_gettuple", "dann_scan_gettuple_many",
     "dann_coalescer_gettuple", "dann_scan_stats", "dann_scan_workspace", "dann_scan_end", "dann_search_batch", "dann_search_batch_device",
+    "dann_scan_fetch",
     "dann_search_batch_mixed", "dann_search_batch_mixed_device", "dann_group_search_batch_mixed",
     "dann_prepare_queries", "dann_code_stride", "dann_sbq_distance", "dann_full_distance",
     "dann_kernel_launches", "dann_last_batch_timing",
@@ -126,6 +127,7 @@ def load_library(path: Optional[str] = None):
     lib.dann_scan_begin.argtypes = [vp, C.POINTER(vp)]
     lib.dann_scan_rescan.argtypes = [vp, vp, vp, C.c_int, C.c_int, C.c_int]
     lib.dann_scan_gettuple.argtypes = [vp, u32p, C.POINTER(C.c_uint16), u32p, C.POINTER(C.c_float)]
+    lib.dann_scan_fetch.argtypes = [vp, C.c_int, vp, vp, vp, vp, vp]
     lib.dann_scan_gettuple_many.argtypes = [vp, C.c_int, vp, vp, vp, vp, vp]
     lib.dann_scan_stats.argtypes = [vp, C.POINTER(_QueryStats)]
     lib.dann_scan_workspace.argtypes = [vp, C.POINTER(_ScanWorkspace)]
@@ -493,6 +495,22 @@ class IndexScan:
         if rc == 0:
             return None
         return int(b.value), int(o.value), int(n.value), float(d.value)
+
+    def fetch(self, n: int):
+        """The next n rows in one GPU step (dann_scan_fetch): exactly what n gettuple calls give.  Returns numpy arrays
+        block, offset, node, dist of length r <= n (r < n only at end of scan) and a list of r dicts shaped like
+        stats(): the scan's counters after each of those calls."""
+        n = int(n)
+        cap = max(n, 0)
+        b = np.zeros(cap, np.uint32)
+        o = np.zeros(cap, np.uint16)
+        nd = np.zeros(cap, np.uint32)
+        d = np.zeros(cap, np.float32)
+        st = np.zeros(cap, STATS_DTYPE)
+        r = _check(self._lib, self._lib.dann_scan_fetch(self._h, n, _np_ptr(b), _np_ptr(o), _np_ptr(nd), _np_ptr(d),
+                                                         _np_ptr(st)))
+        stats = [{k: int(row[k]) for k in STATS_DTYPE.names} for row in st[:r]]
+        return b[:r], o[:r], nd[:r], d[:r], stats
 
     def stats(self) -> dict:
         st = _QueryStats()
